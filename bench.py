@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — IQ Msamples/s demodulated (BASELINE.json metric) on N B200s, one process per GPU.
+"""bench.py — IQ Msamples/s demodulated (BASELINE.json metric) on N H100s, one process per GPU.
 
 A *launch* is one pass of the hot path over one batch: for every one of the GPU's receivers, the next
 `--buffers` reference buffers of 65536 samples (128 KiB mag_buf, `--sdr-buffer-size=128`) of its synthetic
@@ -26,10 +26,7 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import shutil
-import subprocess
 import sys
-import tempfile
 import threading
 import time
 from concurrent.futures import ThreadPoolExecutor
@@ -61,6 +58,8 @@ def parse_args():
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[1] latency leg, the configs[4] leg and the oracle comparison")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last launch returned to its caller "
+                    "(frames, per-buffer results, receiver counters) as DIR/<name>.npy, for comparing two builds output for output")
     return ap.parse_args()
 
 
@@ -208,7 +207,7 @@ def workload_config(args, n_gpus):
             "parallelism": f"{n_gpus} independent GPU(s), streams sharded {args.streams}/GPU, no collective",
             "pipelining": f"value: {args.depth or PIPE_DEPTH} steps in flight per GPU (run_device_uc8_async/wait); e2e: {args.depth or PIPE_DEPTH} steps in flight (run_host_uc8_async/wait: pinned host slab -> H2D on the library's copy stream, overlapping the previous steps' kernels); all results collected on the host inside the timed region",
             "l2": f"device inputs cycle through a ring of {args.ring} distinct steps "
-                  f"({args.ring * args.streams * args.buffers * BUF * 2 / 2**20:.0f} MiB per GPU, L2 is 126 MB); each step reads bytes not touched for {args.ring - 1} steps"}
+                  f"({args.ring * args.streams * args.buffers * BUF * 2 / 2**20:.0f} MiB per GPU, L2 is 50 MB on an H100); each step reads bytes not touched for {args.ring - 1} steps"}
 
 
 def usable_cores() -> int:
@@ -288,51 +287,6 @@ class NvmlClockSampler:
         self.stop_flag = True
         if self.thread:
             self.thread.join(timeout=2)
-
-
-class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
-    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
-        "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
-
-    def __init__(self, gpu_index: int):
-        self.path = tempfile.NamedTemporaryFile(prefix="clocks_", suffix=".csv", delete=False).name
-        self.proc = None
-        self.idx = gpu_index
-
-    def start(self):
-        if shutil.which("nvidia-smi"):
-            self.fh = open(self.path, "w")
-            self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-lms", "100", "-i", str(self.idx)],
-                                         stdout=self.fh, stderr=subprocess.DEVNULL)
-
-    def stop(self) -> dict:
-        out = {"sm_mhz": None, "sm_max_mhz": None, "reasons": []}
-        if not self.proc:
-            return out
-        self.proc.terminate()
-        try:
-            self.proc.wait(timeout=5)
-        except Exception:
-            self.proc.kill()
-        self.fh.close()
-        sm, mx, reasons = [], [], set()
-        names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
-        for ln in open(self.path):
-            f = [x.strip() for x in ln.split(",")]
-            if len(f) < 9:
-                continue
-            try:
-                sm.append(float(f[1])); mx.append(float(f[2]))
-            except ValueError:
-                continue
-            for name, v in zip(names, f[5:9]):
-                if v.lower().startswith("active"):
-                    reasons.add(name)
-        os.unlink(self.path)
-        if sm:
-            out = {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons), "samples": len(sm)}
-        return out
 
 
 def _worker_time_buffers(task):
@@ -473,6 +427,38 @@ def dense_leg(local, args, hbm_peak):
             "roofline_frac": ALG_BYTES_PER_SAMPLE * step_samples / scan_s / 1e9 / hbm_peak}
 
 
+DUMP_ROWS = 100_000              # --dump-outputs: at most this many frames and buffer results (a seeded sample beyond), < 64 MB in all
+
+
+def dump_outputs(d, n_streams: int, out_dir: str) -> dict:
+    """What a caller of the timed path receives from its last launch, for every receiver: the frames (b200_demod_fetch), the
+    per-buffer results (b200_demod_buffer_results) and the cumulative counters (b200_demod_get_stats), one float64 array per
+    field (exact for integers below 2^53).  `<kind>_stream` holds the receiver index of each row."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {}
+    for kind, fetch in (("frames", d.frames), ("buffers", d.buffer_results)):
+        per = [fetch(s) for s in range(n_streams)]
+        rows = np.concatenate(per)
+        stream = np.repeat(np.arange(n_streams), [len(p) for p in per])
+        if len(rows) > DUMP_ROWS:
+            keep = np.sort(np.random.default_rng(0).choice(len(rows), DUMP_ROWS, replace=False))
+            rows, stream = rows[keep], stream[keep]
+        arrays[f"{kind}_stream"] = stream
+        for name in rows.dtype.names:
+            if name != "pad_":
+                arrays[f"{kind}_{name}"] = rows[name]
+    stats = [d.stats(s) for s in range(n_streams)]
+    for name in stats[0]:
+        arrays[f"stats_{name}"] = [st[name] for st in stats]
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        np.save(out / f"{name}.npy", a)
+        total += a.nbytes
+    return {"dir": str(out), "arrays": len(arrays), "bytes": total}
+
+
 def parity_leg(local, args, host, dev_ptr, stride):
     """The timed configuration's first launch (all receivers, device-resident, fresh context) against the CPU oracle, frame for frame
     (outside every timed region; the oracle is the checker here, nothing more)."""
@@ -604,6 +590,9 @@ def b200_arm(args, rank, world, local):
     k_first = 26 + args.warmup * LPS
     ms, scan_ms, launches, frames, clocks = timed(device_step_async, args.steps * LPS, k_first, pipelined=True, sample=True)
     value = world * step_samples * args.steps / (ms * 1e-3) / 1e6
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(d, S, args.dump_outputs)
 
     # --- e2e: host buffers through the C ABI ----------------------------------------------------------------------
     e2e = None
@@ -635,7 +624,7 @@ def b200_arm(args, rank, world, local):
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         peaks = json.loads(pk.read_text())
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     if rank == 0 and not args.no_extra:
         d.close()
         for name, fn in (("config2_single_stream", lambda: latency_leg(local, hbm_peak, cpu_pool)),
@@ -676,13 +665,15 @@ def b200_arm(args, rank, world, local):
         "burst": burst,
         "roofline": {"bound": "hbm", "kernel": "scan_kernel", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
                      "frac": achieved / hbm_peak, "traffic": traffic, "traffic_source": traffic_note,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "H100 SXM data sheet, 3350 GB/s (not a measured peak)",
                      "kernel_ms_per_launch": scan_avg_s * 1e3, "kernel_ms_per_launch_overlapped_with_stage_b": scan_ms / (args.steps * LPS),
                      "timed_in": f"{n_alone} blocking device-resident launches after the value run (kernel alone on the GPU), CUDA events around the launch on its stream",
                      "algorithmic_bytes_per_launch": ALG_BYTES_PER_SAMPLE * launch_samples, "clocks": clk_r},
         "gpu_launches": launches,
         "clocks": clocks,
     }
+    if dumped:
+        line["dumped_outputs"] = dumped
     if e2e:
         line["e2e"] = e2e
     if extra:

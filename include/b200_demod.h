@@ -1,5 +1,5 @@
 /*
- * b200_demod.h — C ABI of the Blackwell-native Mode-S demodulator.
+ * b200_demod.h — C ABI of the Hopper-native Mode-S demodulator.
  *
  * This library replaces exactly one path of wiedehopf/readsb: the 2.4 MSPS Mode-S
  * demodulator (uc8 IQ -> magnitude -> preamble detect -> 5-phase bit slice ->
@@ -20,7 +20,7 @@
  *
  * All entry points are plain C (extern "C"), take plain pointers and sizes, and return 0 on
  * success or a negative B200_E_* code; b200_demod_last_error() gives the text.  There is no CPU
- * fallback: if no sm_100-class CUDA device is usable, b200_demod_create() fails.
+ * fallback: if no sm_90 (H100-class) CUDA device is usable, b200_demod_create() fails.
  */
 #ifndef B200_DEMOD_H
 #define B200_DEMOD_H

@@ -1,4 +1,4 @@
-"""readsb_b200 — Blackwell-native Mode-S demodulator behind readsb's demodulate2400() boundary.
+"""readsb_b200 — Hopper-native Mode-S demodulator behind readsb's demodulate2400() boundary.
 
 Only the hot path lives here: `csrc/` (CUDA kernels + the C ABI declared in include/b200_demod.h),
 `demod.py` (host-side mirror of the reference interface over that C ABI), `synth/` (synthetic

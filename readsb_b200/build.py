@@ -1,7 +1,7 @@
-"""In-tree builds: the CUDA/C-ABI library (nvcc, sm_100a) and the synthetic generator (gcc).
+"""In-tree builds: the CUDA/C-ABI library (nvcc, sm_90a) and the synthetic generator (gcc).
 
-Everything is built next to its sources so the artefacts travel with a repo snapshot
-(.so files are git-ignored, not gpurun-ignored).
+Everything is built next to its sources, so the package is importable from the tree it was built in
+(.so files are git-ignored).
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ LIB_DEMOD = PKG / "libb200demod.so"
 LIB_SYNTH = PKG / "libmodes_synth.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O2,-Wall,-fvisibility=hidden",
     "--fmad=false",            # the LUT arithmetic must not contract mul+add (convert.c:49-56)

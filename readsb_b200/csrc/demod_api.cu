@@ -107,8 +107,8 @@ struct PartCal {
 
 struct b200_demod_ctx {
     b200_demod_config cfg;
-    int device = 0, n_sm = 148;
-    int n_sm_scan = 148;              // CTAs of the persistent scan kernel (one per SM) in blocking runs
+    int device = 0, n_sm = 0;
+    int n_sm_scan = 0;                // CTAs of the persistent scan kernel (one per SM) in blocking runs
     // Pipelined steps: how the SMs are shared between the scan of step n+1 and stage B + finalizer of step n (tune_partition)
     int part_n = 0;                   // CTAs of the scan kernel in pipelined runs; 0 = the whole chip (the two alternate on all SMs)
     bool part_debug = false;
@@ -116,7 +116,7 @@ struct b200_demod_ctx {
     PartCal cal;
     int cal_restarts = 0;
     int scan_sub = 1;                 // chunks per warp when a run is small enough for one CTA per tile (scan_kernel.cu, finish_shared_tile); B200_SCAN_SUB: 0 = whole tiles
-    int n_sm_scan_async = 148;        // ... in pipelined runs, unless the session's measurement chose fewer (part_n, tune_partition) or B200_SCAN_SMS fixed it
+    int n_sm_scan_async = 0;          // ... in pipelined runs, unless the session's measurement chose fewer (part_n, tune_partition) or B200_SCAN_SMS fixed it
     cudaStream_t stream = nullptr, own_stream = nullptr, res_stream = nullptr, copy_stream = nullptr, in_stream = nullptr;
     std::string err;
 
@@ -334,7 +334,8 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
     CUC(cudaSetDevice(dev));
     cudaDeviceProp prop;
     CUC(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) { fail(nullptr, B200_E_NODEV, "device %d is sm_%d%d; the kernels are built for sm_100a only", dev, prop.major, prop.minor); b200_demod_destroy(c); return B200_E_NODEV; }
+    // sm_90a code runs on compute capability 9.0 and nothing else (arch-specific features are not forward compatible)
+    if (prop.major != 9 || prop.minor != 0) { fail(nullptr, B200_E_NODEV, "device %d is sm_%d%d; the kernels are built for sm_90a only", dev, prop.major, prop.minor); b200_demod_destroy(c); return B200_E_NODEV; }
     c->n_sm = prop.multiProcessorCount;
     c->n_sm_scan = c->n_sm;
     // Pipelined steps start with the whole chip for the scan; the session then measures whether a smaller grid - stage B + finalizer
@@ -957,11 +958,10 @@ API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, ui
 // Pipelined steps keep three kernels' worth of work in flight: the scan of step n+1 (one persistent CTA per SM, the whole SM each)
 // and stage B + finalizer of step n (one CTA of 8 warps per receiver, two per SM, latency-bound: a third of the issue slots).
 // Launched over the whole chip they take turns on all SMs.  With a scan grid smaller than the chip the scan runs back to back on
-// its SMs and stage B lives on the rest, in several waves.  Measured on 148 SMs (tools/gpu_partition.sh, bench workload, ms per
-// launch): 148 -> 0.488, 140 -> 0.507, 132 -> 0.520 (stage B does not fit into what is left and holds the scans up: worse than
-// taking turns), 126 -> 0.469, 124 -> 0.476, 120 -> 0.490 (it fits: the step costs what the scan costs on its SMs); the dense
-// stress: 148 -> 1.140, 126 -> 1.232 (stage B is a third of the step there and wants the whole chip).  Where the edge lies depends
-// on the workload, and the kernels' event times say little while they overlap, so a pipelined session MEASURES it: after its first
+// its SMs and stage B lives on the rest, in several waves.  Which is faster depends on whether stage B fits into the SMs the scan
+// leaves free (then the step costs what the scan costs on its SMs) or holds the scans up (then taking turns is better), and on the
+// workload: on the dense stress stage B is a large share of the step and wants the whole chip (tools/gpu_partition.sh times fixed
+// grids).  The kernels' event times say little while they overlap, so a pipelined session MEASURES it: after its first
 // steps it runs with the whole chip, then with 85 % and 82 % of the SMs for the scan (twelve step periods each: host clock between
 // completed steps, the longest dropped), measures the winner once more and keeps it - the whole chip unless a partition wins by
 // 1.5 % and again by 1 %.  A run of a different size (tiles +- 1/8) starts over, up to four times per session.

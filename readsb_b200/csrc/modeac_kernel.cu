@@ -125,8 +125,8 @@ __global__ void modeac_noise_kernel(const AcScanParams P) {
 //             on packed 16-bit halves -> a bit per position; F2 must pass the same test 48 or 49 positions on -> 3 % candidates
 //   front     the candidates 32 at a time: level against the buffer's noise floor, clock phase, F2 tests (:641-672) -> < 1 %
 //   bits      those few: 20 bit cells against the thresholds, framing (:674-731) -> the position's bit in the map
-// (The block-phased predecessor - load a quad, barrier, F1 tests, barrier, F2 / bit cells, barrier - took 0.58 ms per 134 M
-// samples at 2.6 warp instructions per sample; see profiles/.)
+// (A block-phased predecessor - load a quad, barrier, F1 tests, barrier, F2 / bit cells, barrier - needed more than twice the warp
+// instructions per sample.)
 #define AC2_WARPS 28
 #define AC2_BEHIND 8
 #define AC2_AHEAD 104

@@ -51,7 +51,7 @@ __device__ __forceinline__ bool ref_resize_due(uint32_t count, uint32_t bits) { 
 __device__ __forceinline__ bool ref_shrink_due(uint32_t count, uint32_t bits) { return count < (1u << bits) / 9u && bits > ICAO_MINBITS; }
 
 #define RS_WARPS 8            // warps per receiver: buffers of one receiver are resolved speculatively in parallel, eight at a time.
-                              // 128 registers per thread: two CTAs per SM, so 256 receivers are one wave on 148 SMs
+                              // 128 registers per thread: two CTAs per SM, so 256 receivers are one wave on 132 SMs (H100 SXM)
 #define RS_STAGE 384          // PosEntry / score keys of one quad staged in shared memory (denser quads are read in place)
 #define RS_RING  2            // staging buffers per warp: the current quad plus one in flight
 #define NEW_CAP  24           // addresses one buffer may learn in deferred mode before it has to be redone in direct mode

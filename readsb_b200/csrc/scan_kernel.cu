@@ -1,5 +1,5 @@
 // scan_kernel.cu — stage A of the Mode-S demodulator, warp-autonomous version: the stateless, data-parallel part of
-// demodulate2400() as one persistent sm_100a kernel in which EVERY WARP owns whole tiles and never meets a block barrier.
+// demodulate2400() as one persistent sm_90a kernel in which EVERY WARP owns whole tiles and never meets a block barrier.
 //
 // One CTA per SM shares the read-only tables (folded uc8 magnitude table 32 KB, CRC table, single-bit syndromes); each of
 // its warps pulls tiles of SCAN_TILE positions from an atomic counter and walks them in chunks of 512 positions
@@ -27,8 +27,8 @@
 #include "common.h"
 #include "device_utils.cuh"
 
-// Trip counters for the instruction model in profiles/ (tools/scan_model.py): compiled in only with -DB200_SCAN_COUNTERS, which
-// only an analysis build of the test infrastructure passes; nothing of this is in the sm_100a library (its SASS is unchanged).
+// Trip counters for the instruction model of tools/scan_model.py: compiled in only with -DB200_SCAN_COUNTERS, which
+// only an analysis build of the test infrastructure passes; nothing of this is in the sm_90a library (its SASS is unchanged).
 #ifdef B200_SCAN_COUNTERS
 extern "C" { __attribute__((visibility("default"))) unsigned long long b200_scan_counters[16]; }
 #define SCAN_COUNT(id, n) do { if ((threadIdx.x & 31) == 0) b200_scan_counters[id] += (n); } while (0)
@@ -42,7 +42,7 @@ enum { SCN_RUNS, SCN_LOOP_ITERS, SCN_WINDOW_CHUNKS, SCN_FAST_CONVERTS, SCN_EDGE_
 #define SC_WARPS 28
 #endif
 #ifndef SC_MAXNREG
-#define SC_MAXNREG 72                         // SC_WARPS x 32 x SC_MAXNREG <= 65536 registers per SM (28 warps x 72: measured best of 20..32 warps x 64..96)
+#define SC_MAXNREG 72                         // SC_WARPS x 32 x SC_MAXNREG <= 65536 registers per SM (tools/gpu_variants.sh times other splits)
 #endif
 #define CHUNK 512
 #define TILE_CHUNKS (SCAN_TILE / CHUNK)       // 4 chunks of positions per tile

@@ -4,7 +4,7 @@
 readsb frontend calls its converter and publishes a mag_buf (sdr_ifile.c:241-259), `submit_mag`
 + `run` + `frames` stand where the decode thread calls demodulate2400(buf) (readsb.c:871) and the
 frames reach netUseMessage().  There is no CPU implementation behind this class: if the CUDA
-library is missing or no B200-class device is present, construction raises.
+library is missing or no H100-class (sm_90) device is present, construction raises.
 """
 from __future__ import annotations
 
@@ -30,7 +30,7 @@ def lib():
         import os
         path = Path(os.environ.get("B200_DEMOD_LIB") or LIB_PATH)     # an experimental build variant of the same library (build.py)
         if not path.exists():
-            raise DemodError(f"{path} is missing: run `python -m readsb_b200.build` (nvcc, sm_100a). "
+            raise DemodError(f"{path} is missing: run `python -m readsb_b200.build` (nvcc, sm_90a). "
                              "There is no CPU fallback for the demodulator.")
         L = C.CDLL(str(path))
         vp, u32, i64, u64 = C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64

@@ -10,7 +10,7 @@ sys.path.insert(0, str(ROOT / "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 def _cuda_available() -> bool:
@@ -23,7 +23,7 @@ def _cuda_available() -> bool:
 
 def emulated() -> bool:
     """B200_EMU=1: the gpu-marked tests run against the kernels' source compiled for the CPU under the SIMT emulator
-    (tests/emu/, test infrastructure; see tests/test_emu_kernels.py) instead of the sm_100a library on a GPU."""
+    (tests/emu/, test infrastructure; see tests/test_emu_kernels.py) instead of the sm_90a library on a GPU."""
     return os.environ.get("B200_EMU") == "1"
 
 

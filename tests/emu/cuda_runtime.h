@@ -4,7 +4,7 @@
 // change can be checked for logic errors before GPU minutes are spent on it.
 //
 // This is NOT a product path: nothing under readsb_b200/ or include/ refers to it, the product library is still built by
-// nvcc for sm_100a only and still has no CPU path (tests/test_abi.py).  The emulated library is built by
+// nvcc for sm_90a only and still has no CPU path (tests/test_abi.py).  The emulated library is built by
 // tests/emu/build_emu.py into tests/emu/_build/ and is only ever loaded by tests/test_emu_kernels.py.
 //
 // Model: a CTA's threads are fibers scheduled cooperatively on the calling OS thread; CTAs of a grid run one after the

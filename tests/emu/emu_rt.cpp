@@ -218,7 +218,7 @@ cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
     memset(p, 0, sizeof *p);
     snprintf(p->name, sizeof p->name, "SIMT emulator (tests/emu)");
-    p->major = 10; p->minor = 0;
+    p->major = 9; p->minor = 0;
     const char *e = getenv("B200_EMU_SMS");
     p->multiProcessorCount = e ? atoi(e) : 2;      // grid sizes follow the SM count: keep emulated grids small
     if (p->multiProcessorCount < 1) p->multiProcessorCount = 1;

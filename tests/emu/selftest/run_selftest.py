@@ -38,13 +38,13 @@ def make_input():
     return inp
 
 
-def build_sm100a() -> Path:
+def build_sm90a() -> Path:
     """The same source as real CUDA (for the gpu-marked test that pins the emulator's definitions against the hardware)."""
-    out = build_emu.BUILD / "libemu_selftest_sm100a.so"
+    out = build_emu.BUILD / "libemu_selftest_sm90a.so"
     build_emu.BUILD.mkdir(parents=True, exist_ok=True)
     import shutil
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-shared", "-Xcompiler", "-fPIC", "-cudart", "shared",
+    subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-shared", "-Xcompiler", "-fPIC", "-cudart", "shared",
                     str(HERE / "selftest.cu"), "-o", str(out)], check=True)
     return out
 

@@ -61,6 +61,20 @@ def sc16_vectors():
     print("sc16_converters", {k: v.shape for k, v in out.items()})
 
 
+CONFIG1_CAPTURE = dict(seed=2024, frames_per_sec=180.0, df_mask=synth.DF17 | synth.DF11 | synth.AP, n_icao=64, p_bit_error=0.1)
+
+
+def config1_frames():
+    """The reference's frames for tests/test_gpu_fullsize.py::test_config1_ten_second_replay (its 10 s capture is regenerated
+    from the seed there, so only the frames are stored)."""
+    iq = synth.generate(24_000_000, **CONFIG1_CAPTURE)
+    frames = Reference().run_stream(iq, 131072, cap=8192)[0]
+    (HERE / "replay").mkdir(exist_ok=True)
+    np.savez_compressed(HERE / "replay" / "config1_10s.npz", frames=frames)
+    print("config1_10s", len(frames), "frames")
+
+
 if __name__ == "__main__":
     main()
     sc16_vectors()
+    config1_frames()

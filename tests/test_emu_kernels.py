@@ -5,9 +5,9 @@ memory, inline PTX) with g++ against a SIMT emulator — one fiber per CUDA thre
 rendezvous points — and the gpu-marked parity tests are then run against that library through the same C ABI and the same
 Python mirror.  This is TEST INFRASTRUCTURE: it checks the kernels' logic where no GPU is available (this tier runs without
 one) and lets a kernel change be tried before GPU minutes are spent on it.  It is not a product path — the product library is
-built by nvcc for sm_100a only, has no CPU path (tests/test_abi.py) and never loads the emulated one — and it says nothing
+built by nvcc for sm_90a only, has no CPU path (tests/test_abi.py) and never loads the emulated one — and it says nothing
 about performance, memory-ordering races between warps, or anything else that only exists on the hardware: the gpu-marked
-tests on a B200 remain the parity tests proper.
+tests on an H100 remain the parity tests proper.
 """
 import os
 import subprocess

@@ -1,7 +1,7 @@
 """Pins the SIMT emulator's definitions (tests/emu/, test infrastructure) against the hardware: tests/emu/selftest/selftest.cu
 exercises every primitive the emulator provides — shuffles, ballot, REDUX, popc / ffs / clz / brev, funnel shifts, byte_perm,
 prmt in sign-replication mode, dp2a.lo / .hi, mad.wide, cp.async, shared / global atomics, __syncthreads, reconvergence at a
-__syncwarp — and is valid CUDA: built by nvcc for sm_100a and run on the GPU it must give the results the emulated build gives
+__syncwarp — and is valid CUDA: built by nvcc for sm_90a and run on the GPU it must give the results the emulated build gives
 (both are checked against the same numpy expectations, written from the CUDA / PTX definitions)."""
 import ctypes
 import os
@@ -26,7 +26,7 @@ def test_emulator_primitives_match_the_hardware(cuda):
     else:
         import torch
         try:
-            lib = st.build_sm100a()
+            lib = st.build_sm90a()
         except (OSError, FileNotFoundError) as e:           # no nvcc on this box: nothing to compare with
             pytest.skip(f"nvcc not available: {e}")
         L = ctypes.CDLL(str(lib))

@@ -377,7 +377,7 @@ def main():
     ap.add_argument("--cases", type=int, default=50)
     ap.add_argument("--minutes", type=float, default=0.0, help="stop after this many minutes (0 = run all cases)")
     ap.add_argument("--only", type=int, default=-1)
-    ap.add_argument("--emu", type=int, default=1, help="1: the emulated library (default), 0: the sm_100a library on a GPU")
+    ap.add_argument("--emu", type=int, default=1, help="1: the emulated library (default), 0: the sm_90a library on a GPU")
     ap.add_argument("-v", action="store_true")
     a = ap.parse_args()
     if a.emu:

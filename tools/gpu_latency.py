@@ -4,7 +4,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 import bench
-print(json.dumps(bench.latency_leg(0, 6489.0, None), indent=1))
+print(json.dumps(bench.latency_leg(0, 3350.0, None), indent=1))
 
 import ctypes as C, os
 from readsb_b200.demod import lib

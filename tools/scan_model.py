@@ -1,5 +1,5 @@
 """Instruction model of scan_kernel: dynamic trip counts (from the kernels' source run under the SIMT emulator with
--DB200_SCAN_COUNTERS, tests/emu/) x static SASS instruction counts per section (nvdisasm of the sm_100a cubin, inline chains
+-DB200_SCAN_COUNTERS, tests/emu/) x static SASS instruction counts per section (nvdisasm of the sm_90a cubin, inline chains
 resolved; numbers below were read off HEAD's cubin — re-derive them with `nvdisasm --print-line-info-inline` after changing
 the kernel).  TEST / ANALYSIS TOOLING; says where the warp instructions go, not how long they take.
 

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Everything that can be checked without a GPU, in one go (about 10 minutes on 8 cores):
-#   build (nvcc cross-compile for sm_100a, oracle, reference pair), the not-gpu tier (which includes the emulated kernels under the
+#   build (nvcc cross-compile for sm_90a, oracle, reference pair), the not-gpu tier (which includes the emulated kernels under the
 #   gpu-marked tests, ASan, UBSan, two random schedules, allocation-fault injection), a fuzz campaign, the instruction model.
 set -e
 cd "$(dirname "$0")/.."
