@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(BEAST_THREADS) beast_encode_kernel(const Beast
     const uint32_t b0 = P.segs[sb].first_buf, b1 = P.segs[se - 1].first_buf + P.segs[se - 1].n_bufs;
     uint32_t running = 0;
     for (int pass = 0; pass < 2; pass++) {
-        uint32_t fcur = P.frame_prefix[s];
+        uint32_t fcur = P.frame_span[2 * s];
         running = 0;
         for (uint32_t b = b0; b < b1; b++) {
             const uint32_t nf = P.buf_out[b].n_frames;

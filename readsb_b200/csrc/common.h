@@ -125,7 +125,11 @@ struct RunCtl {
     uint32_t total_frames;
     uint32_t stage_need;     // with overflow bit1: the largest number of live records one tile produced (staging areas too small)
     uint32_t pad_[2];
+    uint32_t cap_check;      // stage B's capacity check of this run (resolve_kernel): 0 not yet, 1 in progress, CAP_GO / CAP_STOP made
+    uint32_t pad1_[3];
 };
+#define CAP_STOP 2u          // cap_check: made, stage B must not run (this step is going to be repeated)
+#define CAP_GO   3u          // cap_check: made, stage B runs
 
 #define RUN_REPEAT_BITS (1u | 2u | 8u | 16u)   // stage B did not run (or must not): the host repairs and repeats the step
 
@@ -170,13 +174,11 @@ struct FinalizeParams {
     const uint32_t *stream_seg_begin;
     uint32_t n_streams;
     b200_frame *frames;
-    const uint32_t *frame_count;
-    const uint32_t *frame_prefix;     // exclusive prefix of frame_count (device computed)
-    uint32_t *frame_prefix_out;       // the same array, for the one-receiver launch that computes it itself
+    uint32_t *frame_span;             // [n_streams][2]: where the receiver's frames start in `packed`, and how many there are
     Segment one_seg;                  // (see ScanParams) the run's only segment, when one_seg_valid
     uint32_t one_seg_valid;
     uint32_t frame_cap;
-    b200_frame *packed;               // all frames of the run, stream-major
+    b200_frame *packed;               // all frames of the run: each receiver's in order, in one contiguous range (frame_span)
     const Rec *rec_pool;
     BufAcc *buf_acc;
     StreamState *state;
@@ -195,17 +197,17 @@ struct ResolveParams {
     b200_buffer_result *buf_out;      // per run buffer results (n_frames, flip flag, ...)
     StreamState *state;
     b200_frame *frames;               // [n_streams][frame_cap]
-    uint32_t *frame_count;            // [n_streams]
     uint32_t frame_cap;
     uint32_t per_buf_cap;             // frames one reference buffer can hold (buf_samples / 113 + 2); frame_cap = buffers per run x this
     RunCtl *ctl;
-    const RunCtl *prev_ctl;           // asynchronous pipeline: control block of the step ahead of this one (or nullptr)
+    const uint32_t *prev_stop;        // asynchronous pipeline: the stop_out of the step ahead of this one (or nullptr)
+    uint32_t *stop_out;               // set to 1 when this run's stage B does not run (the run is going to be repeated), else to 0
     int32_t ttl_ms;
     uint32_t *stream_addable;         // [n_streams] upper bound of the filter adds of this run (scan kernel); read and zeroed by the capacity check
     Segment one_seg;                  // (see ScanParams) the run's only segment, when one_seg_valid
     uint32_t one_seg_valid;
-    uint32_t solo;                    // one receiver in the context: capacity check, stage B, frame prefix and finalizer in ONE launch
-    FinalizeParams fin;               // (solo) what the finalizer needs
+    uint32_t solo;                    // one receiver in the context: resolve_solo_kernel (see resolve_kernel.cu)
+    FinalizeParams fin;               // what the finalizer needs
     // (solo, optional) the kernel PUBLISHES the run's result block itself: copies publish_head bytes + the packed frames from
     // publish_src (device) to publish_dst (the host's pinned copy, mapped into the device's address space) - no device-to-host
     // copy operation in the stream - and then zeroes the control block and the per-buffer sums for the next run (no memset either)
@@ -263,8 +265,8 @@ struct AcWalkParams {
 struct BeastParams {                 // beast_kernel.cu
     const Segment *segs;
     const uint32_t *stream_seg_begin;
-    const b200_frame *frames;         // packed stream-major
-    const uint32_t *frame_prefix;
+    const b200_frame *frames;         // packed (FinalizeParams::packed)
+    const uint32_t *frame_span;       // [stream][2]: first frame, frame count
     const b200_buffer_result *buf_out;
     const b200_modeac *ac;            // packed in buffer order, or null
     const uint32_t *ac_prefix;        // [buffer + 1], or null
@@ -296,7 +298,6 @@ int b200_prepare_scan(void);       // per-device kernel attributes (dynamic shar
 int b200_prepare_resolve(void);
 int b200_prepare_modeac(void);
 int b200_launch_resolve(const ResolveParams *p, int any_grown, void *stream);
-int b200_launch_finalize(const FinalizeParams *p, uint32_t *d_frame_prefix, RunCtl *ctl, int n_sm, void *stream);
 int b200_launch_init_state(StreamState *state, uint32_t n, uint32_t *slab, void *stream);
 int b200_launch_icao_rehash(StreamState *state, uint32_t stream, uint32_t *new0, uint32_t *new1, uint32_t new_log2, void *stream_);
 int b200_launch_modeac(const AcScanParams *sp, const AcWalkParams *wp, int n_sm, void *stream);

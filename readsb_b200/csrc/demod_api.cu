@@ -7,9 +7,9 @@
 //
 // A run owns one SLOT (segment tables, candidate pools, result buffers).  The blocking calls use slot 0 on one
 // CUDA stream.  The asynchronous calls (run_device_uc8_async / run_host_uc8_async / wait) cycle through NSLOT slots: the
-// scan kernels of consecutive steps run back to back on the scan stream, stage B + finalize + D2H of each step follow
-// on the resolve stream (higher priority) as soon as its scan has ended; stage B kernels stay ordered among themselves,
-// which is all the per-receiver state needs.
+// scan kernels of consecutive steps run back to back on the scan stream, stage B (one launch: capacity check, stage B, frame
+// placement, finalizer) + D2H of each step follow on the resolve stream (higher priority) as soon as its scan has ended; stage B
+// kernels stay ordered among themselves, which is all the per-receiver state needs.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -47,7 +47,7 @@ struct Slot {
     // Descriptors of a run travel in ONE host-to-device copy and its results in ONE device-to-host copy: two blocks per slot, laid
     // out per run (layout_run); the d_* / h_* members below point into them.
     //   descriptor block  [stream_seg_begin (S+1) | segs (nseg) | tile_seg (ntile)]
-    //   result block      [RunCtl | buf_acc (nbuf) | frame_prefix (S+1) | buf_out (nbuf) | packed frames ...]
+    //   result block      [RunCtl | buf_acc (nbuf) | frame_span (2S) | buf_out (nbuf) | packed frames ...]
     uint8_t *d_desc = nullptr, *h_desc = nullptr, *d_res = nullptr, *h_res = nullptr;
     uint8_t *d_res_host = nullptr;    // h_res as the device sees it (mapped pinned memory): the one-receiver kernel publishes its results there
     bool res_clean = false;           // RunCtl + BufAcc[] in d_res are zero (the one-receiver kernel cleans up after itself)
@@ -65,7 +65,7 @@ struct Slot {
     BufAcc *d_buf_acc = nullptr, *h_buf_acc = nullptr;
     b200_buffer_result *d_buf_out = nullptr, *h_buf_out = nullptr;
     b200_frame *d_frames = nullptr, *d_packed = nullptr, *h_packed = nullptr;
-    uint32_t *d_frame_count = nullptr, *d_frame_prefix = nullptr, *h_frame_prefix = nullptr;
+    uint32_t *d_frame_span = nullptr, *h_frame_span = nullptr;    // per receiver: first packed frame, frame count (FinalizeParams)
     uint32_t *d_addable = nullptr;    // [S] filter adds this run can make at most (scan kernel -> capacity check, which zeroes it again)
     // Mode A/C (contexts created with B200_CFG_MODE_AC)
     uint32_t *d_ac_bitmap = nullptr, *d_ac_noise = nullptr;
@@ -140,6 +140,8 @@ struct b200_demod_ctx {
     int next_async = 0;               // slot the next asynchronous step takes
     int head = 0, n_flight = 0;       // oldest step in flight, number of steps in flight (slots head, head+1, ... mod NSLOT)
     uint32_t *d_carry_src = nullptr, *h_carry_src = nullptr;
+    uint32_t *d_stop = nullptr;       // [NSLOT] per slot: 1 when its last run's stage B did not run (ResolveParams::stop_out)
+    uint8_t *h_zero = nullptr;        // pinned zeros: a run's control block and per-buffer sums are cleared by a copy from here (enqueue)
     // scan kernel: per-warp staging of a run's live records, spill of the pre-check queue, ticks of the run in progress
     Rec *d_stage_rec = nullptr; uint32_t *d_stage_key = nullptr; uint16_t *d_q1_over = nullptr; uint32_t *d_tick_scratch = nullptr;
     uint32_t stage_cap = 0;
@@ -220,7 +222,7 @@ static void layout_run(b200_demod_ctx *c, Slot &sl);
 static void free_slot(Slot &s) {
     cudaFree(s.d_desc); cudaFree(s.d_res); cudaFreeHost(s.h_desc); cudaFreeHost(s.h_res); cudaFree(s.d_pos_pool);
     cudaFree(s.d_rec_pool); cudaFree(s.d_key_pool); cudaFree(s.d_tile_out);
-    cudaFree(s.d_frames); cudaFree(s.d_frame_count); cudaFree(s.d_addable);
+    cudaFree(s.d_frames); cudaFree(s.d_addable);
     cudaFree(s.d_mag_copy); cudaFree(s.d_ac_bitmap); cudaFree(s.d_ac_noise); cudaFree(s.d_ac_count); cudaFree(s.d_ac_prefix); cudaFree(s.d_ac_out); cudaFree(s.d_ac_packed);
     cudaFreeHost(s.h_ac_prefix); cudaFreeHost(s.h_ac_packed);
     cudaFree(s.d_ac_levels); cudaFreeHost(s.h_ac_levels);
@@ -239,19 +241,18 @@ static cudaError_t alloc_slot(b200_demod_ctx *c, Slot &s, uint32_t rec_cap) {
     s.h_stream_seg_begin = (uint32_t *)malloc(((size_t)S + 1) * 4);
     if (!s.h_segs || !s.h_tile_seg || !s.h_stream_seg_begin) return cudaErrorMemoryAllocation;
     s.desc_cap = pad16(((size_t)S + 1) * 4) + (size_t)c->seg_cap * sizeof(Segment) + (size_t)c->tile_cap * 4 + 64;
-    s.res_cap = sizeof(RunCtl) + (size_t)c->buf_cap * (sizeof(BufAcc) + sizeof(b200_buffer_result)) + pad16(((size_t)S + 1) * 4)
+    s.res_cap = sizeof(RunCtl) + (size_t)c->buf_cap * (sizeof(BufAcc) + sizeof(b200_buffer_result)) + pad16((size_t)S * 8)
               + (size_t)S * c->frame_cap * sizeof(b200_frame) + 64;
     A(cudaMalloc((void **)&s.d_desc, s.desc_cap)); A(cudaHostAlloc((void **)&s.h_desc, s.desc_cap, cudaHostAllocDefault));
     A(cudaMalloc((void **)&s.d_res, s.res_cap)); A(cudaHostAlloc((void **)&s.h_res, s.res_cap, cudaHostAllocMapped));
     A(cudaHostGetDevicePointer((void **)&s.d_res_host, s.h_res, 0));
     A(cudaMemset(s.d_res, 0, sizeof(RunCtl)));
-    memset(s.h_res, 0, sizeof(RunCtl) + pad16(((size_t)S + 1) * 4));
-    s.d_ctl = reinterpret_cast<RunCtl *>(s.d_res); s.h_ctl = reinterpret_cast<RunCtl *>(s.h_res);     // fixed: the next step reads it as prev_ctl
+    memset(s.h_res, 0, sizeof(RunCtl) + pad16((size_t)S * 8));
+    s.d_ctl = reinterpret_cast<RunCtl *>(s.d_res); s.h_ctl = reinterpret_cast<RunCtl *>(s.h_res);
     A(dev_alloc(&s.d_pos_pool, (size_t)c->tile_cap * SCAN_TILE));
     A(dev_alloc(&s.d_rec_pool, s.rec_cap)); A(dev_alloc(&s.d_key_pool, s.rec_cap));
     A(dev_alloc(&s.d_tile_out, c->tile_cap));
     A(dev_alloc(&s.d_frames, (size_t)S * c->frame_cap));
-    A(dev_alloc(&s.d_frame_count, S)); A(cudaMemset(s.d_frame_count, 0, S * 4));
     A(dev_alloc(&s.d_addable, S)); A(cudaMemset(s.d_addable, 0, S * 4));
 
     if (c->cfg.flags & B200_CFG_MODE_AC) {
@@ -289,7 +290,7 @@ static void layout_run(b200_demod_ctx *c, Slot &sl) {
     sl.desc_bytes = o_tile + (sl.upload_tiles ? (size_t)sl.ntile * 4 : 0);
     size_t r = sizeof(RunCtl);
     sl.d_buf_acc = reinterpret_cast<BufAcc *>(sl.d_res + r); sl.h_buf_acc = reinterpret_cast<BufAcc *>(sl.h_res + r); r += (size_t)sl.nbuf * sizeof(BufAcc);
-    sl.d_frame_prefix = reinterpret_cast<uint32_t *>(sl.d_res + r); sl.h_frame_prefix = reinterpret_cast<uint32_t *>(sl.h_res + r); r += pad16((S + 1) * 4);
+    sl.d_frame_span = reinterpret_cast<uint32_t *>(sl.d_res + r); sl.h_frame_span = reinterpret_cast<uint32_t *>(sl.h_res + r); r += pad16(S * 8);
     sl.d_buf_out = reinterpret_cast<b200_buffer_result *>(sl.d_res + r); sl.h_buf_out = reinterpret_cast<b200_buffer_result *>(sl.h_res + r); r += (size_t)sl.nbuf * sizeof(b200_buffer_result);
     r = pad16(r);
     sl.d_packed = reinterpret_cast<b200_frame *>(sl.d_res + r); sl.h_packed = reinterpret_cast<b200_frame *>(sl.h_res + r);
@@ -302,9 +303,9 @@ API void b200_demod_destroy(b200_demod_ctx *c) {
     cudaDeviceSynchronize();
     cudaFree(c->d_tables); cudaFree(c->d_lut_full); cudaFree(c->d_state); cudaFree(c->d_arena); cudaFree(c->d_icao_slab);
     for (uint32_t *t : c->icao_grown) cudaFree(t);
-    cudaFree(c->d_carry_src); cudaFree(c->d_result);
+    cudaFree(c->d_carry_src); cudaFree(c->d_result); cudaFree(c->d_stop);
     cudaFree(c->d_stage_rec); cudaFree(c->d_stage_key); cudaFree(c->d_q1_over); cudaFree(c->d_tick_scratch);
-    cudaFreeHost(c->h_carry_src);
+    cudaFreeHost(c->h_carry_src); cudaFreeHost(c->h_zero);
     cudaFree(c->d_raw16); cudaFree(c->d_fsum); cudaFreeHost(c->h_fsum);
     cudaFree(c->d_beast); cudaFree(c->d_beast_meta); cudaFreeHost(c->h_beast); cudaFreeHost(c->h_beast_meta);
     for (Slot &sl : c->slot) free_slot(sl);
@@ -381,6 +382,7 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
     CUC(dev_alloc(&c->d_icao_slab, (size_t)S * 2 * ICAO_CAP));
     CUC((cudaError_t)b200_launch_init_state(c->d_state, S, c->d_icao_slab, c->stream));
     CUC(dev_alloc(&c->d_result, 1));
+    CUC(dev_alloc(&c->d_stop, NSLOT)); CUC(cudaMemsetAsync(c->d_stop, 0, NSLOT * 4, c->stream));
 
     // arena for host submits: [326-sample halo][K buffers, each with room for its own halo when magnitudes are submitted]
     c->stream_stride = (((size_t)K * ((size_t)BUF + B200_TRAIL + 16) * 2 + 1024) + 255) & ~(size_t)255;
@@ -406,6 +408,8 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
     const size_t positions = (size_t)S * K * BUF;
     CUC(alloc_slot(c, c->slot[0], (uint32_t)std::max<size_t>(65536, positions / 16)));
     CUC(dev_alloc(&c->d_carry_src, S)); CUC(pin_alloc(&c->h_carry_src, S));
+    CUC(pin_alloc(&c->h_zero, sizeof(RunCtl) + (size_t)c->buf_cap * sizeof(BufAcc)));
+    memset(c->h_zero, 0, sizeof(RunCtl) + (size_t)c->buf_cap * sizeof(BufAcc));
     CUC(cudaStreamSynchronize(c->stream));
 #undef CUC
     *out = c;
@@ -535,20 +539,16 @@ static void add_segment(b200_demod_ctx *c, Slot &sl, uint32_t stream, const uint
     sl.ntile += g.n_tiles; sl.nbuf += n_bufs; sl.nseg++;
 }
 
-// Enqueue one run held by `sl`: tables up, stage A on `scan`, stage B + finalize + first result copy on `res`
-// (the same stream in blocking mode).  `prev_ctl`: control block of the step in flight before this one (async mode).
-static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t res, const RunCtl *prev_ctl) {
+// Enqueue one run held by `sl`: tables up, stage A on `scan`, stage B (with the finalizer) + first result copy on `res`
+// (the same stream in blocking mode).  `prev_stop`: stop word of the step in flight before this one (async mode), see stop_out.
+static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t res, const uint32_t *prev_stop) {
     const uint32_t S = c->cfg.n_streams;
     // The run's descriptors.  Pipelined: they go up on the copy stream right now, while the step before this one is still
     // scanning, so that this step's scan kernel is ready the moment that one ends — together with the other step's stage B,
     // and placed before it (stream priority): one persistent CTA per SM first, stage B's small CTAs into what is left.
+    // (Nothing on the device still reads this slot's blocks: its previous run was collected.  The step after that run learns whether
+    // it has to be skipped from the slot's stop word, which this run's stage B overwrites only after that step's stage B - same stream.)
     cudaStream_t pre = scan != res ? c->copy_stream : scan;
-    if (pre != scan) {
-        // This slot's control block is what the step enqueued after its previous run reads as `prev_ctl`: do not overwrite it before
-        // that step's stage B has looked (it may still be queued behind other work on the resolve stream).
-        Slot &succ = c->slot[((&sl - c->slot) + 1) % NSLOT];
-        if (succ.in_flight) CU(c, cudaStreamWaitEvent(pre, succ.ev[2], 0));
-    }
     layout_run(c, sl);
     // One receiver, one segment, no Mode A/C (the drop-in's call shape): the descriptor rides in the kernel parameters
     const bool one_seg = S == 1 && sl.nseg == 1 && !(c->cfg.flags & B200_CFG_MODE_AC) && scan == res;
@@ -559,8 +559,10 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     // block and the per-buffer sums when it is done - no memset, no device-to-host copy in the stream.
     const bool publish = S == 1 && !(c->cfg.flags & B200_CFG_MODE_AC) && scan == res;
     const bool timing = !((c->cfg.flags & B200_CFG_NO_TIMING) && scan == res);
+    // Control block + per-buffer sums: zeroed by a copy engine.  (A memset runs on the SMs, and while the step before this one keeps
+    // them busy it would hold this step's scan kernel back.)
     if (!(publish && sl.res_clean))
-        CU(c, cudaMemsetAsync(sl.d_res, 0, sizeof(RunCtl) + (size_t)sl.nbuf * sizeof(BufAcc), pre));       // control block + per-buffer sums
+        CU(c, cudaMemcpyAsync(sl.d_res, c->h_zero, sizeof(RunCtl) + (size_t)sl.nbuf * sizeof(BufAcc), cudaMemcpyHostToDevice, pre));
     sl.res_clean = false; sl.published = publish; sl.timed = timing;
     if (pre != scan) { CU(c, cudaEventRecord(sl.ev[7], pre)); CU(c, cudaStreamWaitEvent(scan, sl.ev[7], 0)); }
     sl.launches = 0;
@@ -605,15 +607,15 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
 
     FinalizeParams fp;
     fp.segs = sl.d_segs; fp.stream_seg_begin = sl.d_stream_seg_begin; fp.n_streams = S; fp.frames = sl.d_frames;
-    fp.frame_count = sl.d_frame_count; fp.frame_prefix = sl.d_frame_prefix; fp.frame_prefix_out = sl.d_frame_prefix; fp.frame_cap = c->frame_cap; fp.packed = sl.d_packed;
+    fp.frame_span = sl.d_frame_span; fp.frame_cap = c->frame_cap; fp.packed = sl.d_packed;
     fp.buf_acc = sl.d_buf_acc; fp.state = c->d_state; fp.lut_full = c->d_lut_full; fp.rec_pool = sl.d_rec_pool;
     fp.one_seg = sp.one_seg; fp.one_seg_valid = sp.one_seg_valid;
-    const bool solo = S == 1;          // one receiver: stage B, frame prefix and finalizer are one launch (resolve_kernel, solo)
+    const bool solo = S == 1;          // one receiver: resolve_solo_kernel (also publishes its results / carries the halo)
     ResolveParams rp;
     rp.segs = sl.d_segs; rp.stream_seg_begin = sl.d_stream_seg_begin; rp.n_streams = S; rp.pos_pool = sl.d_pos_pool;
     rp.rec_pool = sl.d_rec_pool; rp.key_pool = sl.d_key_pool; rp.tile_out = sl.d_tile_out; rp.buf_acc = sl.d_buf_acc; rp.buf_out = sl.d_buf_out;
-    rp.state = c->d_state; rp.frames = sl.d_frames; rp.frame_count = sl.d_frame_count; rp.frame_cap = c->frame_cap; rp.per_buf_cap = c->cfg.buf_samples / 113 + 2;
-    rp.ctl = sl.d_ctl; rp.prev_ctl = prev_ctl; rp.ttl_ms = c->cfg.icao_ttl_ms; rp.stream_addable = sl.d_addable;
+    rp.state = c->d_state; rp.frames = sl.d_frames; rp.frame_cap = c->frame_cap; rp.per_buf_cap = c->cfg.buf_samples / 113 + 2;
+    rp.ctl = sl.d_ctl; rp.prev_stop = prev_stop; rp.stop_out = c->d_stop + (&sl - c->slot); rp.ttl_ms = c->cfg.icao_ttl_ms; rp.stream_addable = sl.d_addable;
     rp.one_seg = sp.one_seg; rp.one_seg_valid = sp.one_seg_valid;
     rp.solo = solo ? 1u : 0u; rp.fin = fp;
     rp.publish_src = nullptr; rp.publish_dst = nullptr; rp.publish_head = 0; rp.publish_clear = 0;
@@ -627,10 +629,8 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
         rp.publish_head = (uint32_t)sl.res_head; rp.publish_clear = (uint32_t)(sizeof(RunCtl) + (size_t)sl.nbuf * sizeof(BufAcc));
     }
     { const int grown = !c->icao_grown.empty();
-      int r = b200_launch_resolve(&rp, grown, res); if (r) return fail(c, B200_E_CUDA, "resolve launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += solo ? 1 : 2 + grown; }
-    if (timing) CU(c, cudaEventRecord(sl.ev[2], res));
-    if (!solo) { int r = b200_launch_finalize(&fp, sl.d_frame_prefix, sl.d_ctl, c->n_sm, res); if (r) return fail(c, B200_E_CUDA, "finalize launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += 2; }
-    if (timing) CU(c, cudaEventRecord(sl.ev[3], res));
+      int r = b200_launch_resolve(&rp, grown, res); if (r) return fail(c, B200_E_CUDA, "resolve launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += solo ? 1 : 1 + grown; }
+    if (timing) { CU(c, cudaEventRecord(sl.ev[2], res)); CU(c, cudaEventRecord(sl.ev[3], res)); }     // (stage B and finalizer: one launch)
 
     if (mode_ac) {      // per-buffer reply lists -> one packed array in buffer order, receiver statistics
         if (res != scan) CU(c, cudaStreamWaitEvent(res, sl.ev[6], 0));
@@ -651,7 +651,6 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
 // value when the run has to be repeated: 1 = record pool too small, 2 = dense-tile scratch arena needed, 3 = skipped
 // because the step before it had to be repeated, 4 = a receiver's ICAO filter tables have to grow first.
 static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
-    const uint32_t S = c->cfg.n_streams;
     if (sl.timed) CU(c, cudaEventSynchronize(sl.ev[4])); else CU(c, cudaStreamSynchronize(res));
     if (sl.published) sl.res_clean = true;               // the kernel zeroed RunCtl + BufAcc[] after publishing them
     const uint32_t ov = sl.h_ctl->overflow;
@@ -667,7 +666,7 @@ static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
     sl.ms[3] = 0;
     if (mode_ac && sl.timed) cudaEventElapsedTime(&sl.ms[3], sl.ev[1], sl.ev[6]);       // Mode A/C noise + scan + walk kernels
     if (total_ac) CU(c, cudaMemcpyAsync(sl.h_ac_packed, sl.d_ac_packed, (size_t)total_ac * sizeof(b200_modeac), cudaMemcpyDeviceToHost, c->copy_stream));
-    const uint32_t total = sl.h_frame_prefix[S];
+    const uint32_t total = sl.h_ctl->total_frames;
     sl.run_frames = total;
     if (total_ac && total <= sl.first_frames) { CU(c, cudaEventRecord(sl.ev[5], c->copy_stream)); CU(c, cudaEventSynchronize(sl.ev[5])); }
     const bool more_frames = total > sl.first_frames;
@@ -883,7 +882,7 @@ API int b200_demod_run_device_uc8(b200_demod_ctx *c, const uint8_t *d_iq, uint64
 // Enqueues the run built in slot next_async behind the steps already in flight and advances the ring.
 static int launch_async(b200_demod_ctx *c, Slot &sl) {
     Slot &before = c->slot[(c->next_async + NSLOT - 1) % NSLOT];      // the step enqueued just before this one
-    int rc = enqueue(c, sl, c->stream, c->res_stream, before.in_flight ? before.d_ctl : nullptr);
+    int rc = enqueue(c, sl, c->stream, c->res_stream, before.in_flight ? c->d_stop + (&before - c->slot) : nullptr);
     if (rc != B200_OK) return rc;
     if (c->n_flight == 0) c->head = c->next_async;
     sl.in_flight = true; sl.completed = false;
@@ -1045,17 +1044,17 @@ API int b200_demod_total_frames(b200_demod_ctx *c, uint64_t *n) { if (!c || !n) 
 API int b200_demod_frame_count(b200_demod_ctx *c, uint32_t s, uint32_t *n) {
     if (!c || !n || s >= c->cfg.n_streams) return B200_E_INVAL;
     const Slot &sl = c->slot[c->cur];
-    *n = sl.h_frame_prefix[s + 1] - sl.h_frame_prefix[s];
+    *n = sl.h_frame_span[2 * s + 1];
     return B200_OK;
 }
 
 API int b200_demod_fetch(b200_demod_ctx *c, uint32_t s, b200_frame *out, uint32_t cap, uint32_t *n) {
     if (!c || !n || s >= c->cfg.n_streams) return B200_E_INVAL;
     const Slot &sl = c->slot[c->cur];
-    const uint32_t cnt = sl.h_frame_prefix[s + 1] - sl.h_frame_prefix[s];
+    const uint32_t cnt = sl.h_frame_span[2 * s + 1];
     *n = cnt;
     if (cnt > cap) return fail(c, B200_E_OVERFLOW, "stream %u has %u frames, output holds %u", s, cnt, cap);
-    if (cnt) memcpy(out, sl.h_packed + sl.h_frame_prefix[s], (size_t)cnt * sizeof(b200_frame));
+    if (cnt) memcpy(out, sl.h_packed + sl.h_frame_span[2 * s], (size_t)cnt * sizeof(b200_frame));
     return B200_OK;
 }
 
@@ -1097,7 +1096,7 @@ API int b200_demod_fetch_beast(b200_demod_ctx *c, uint32_t s, uint32_t flags, ui
         if (!sl.desc_on_device) { CU(c, cudaMemcpyAsync(sl.d_desc, sl.h_desc, sl.desc_bytes, cudaMemcpyHostToDevice, st)); sl.desc_on_device = true; }
         CU(c, cudaMemsetAsync(c->d_beast_meta, 0, (2 * (size_t)S + 1) * 4, st));
         BeastParams bp;
-        bp.segs = sl.d_segs; bp.stream_seg_begin = sl.d_stream_seg_begin; bp.frames = sl.d_packed; bp.frame_prefix = sl.d_frame_prefix;
+        bp.segs = sl.d_segs; bp.stream_seg_begin = sl.d_stream_seg_begin; bp.frames = sl.d_packed; bp.frame_span = sl.d_frame_span;
         bp.buf_out = sl.d_buf_out; bp.ac = mode_ac ? sl.d_ac_packed : nullptr; bp.ac_prefix = mode_ac ? sl.d_ac_prefix : nullptr;
         bp.out = c->d_beast; bp.stream_off = c->d_beast_meta; bp.stream_len = c->d_beast_meta + S; bp.total = c->d_beast_meta + 2 * S;
         bp.cap = c->beast_cap; bp.verbatim = (flags & B200_BEAST_VERBATIM) ? 1u : 0u;

@@ -7,8 +7,8 @@
 //                   filter generations (icao_filter.c) in shared memory.  The walk touches only staged data:
 //                   each tile's PosEntry list and 32-bit score keys arrive through a cp.async ring three tiles
 //                   ahead, so no dependent global load sits on the sequential path.
-//   finalize_kernel one warp per accepted frame (fully parallel): assembles the frame from its 32-byte record
-//                   (bit fix / DF17 repair, mode_s.c:443-596), signal power (demod_2400.c:436-457), per-buffer /
+//   finalize_stream the same CTA, after its receiver is resolved, one warp per accepted frame: assembles the frame from its
+//                   32-byte record (bit fix / DF17 repair, mode_s.c:443-596), signal power (demod_2400.c:436-457), per-buffer /
 //                   per-receiver power statistics, packing of the frame list for a single D2H copy.
 #include "common.h"
 #include "device_utils.cuh"
@@ -307,7 +307,7 @@ __device__ __forceinline__ void resolve_buffer(const bool DEFER, const ResolvePa
                 const uint32_t j = d - d_begin;
                 const int64_t ts = buf_ts + (int64_t)j * 5 + (8 + 56) * 12 + (4 + best_phase);   // demod_2400.c:406
                 if (nframes < fcap) {
-                    // accept record; finalize_kernel turns it into the full frame from the 32-byte Rec
+                    // accept record; finalize_stream turns it into the full frame from the 32-byte Rec
                     b200_frame fr;
                     fr.timestamp = ts; fr.sigpow_sum = 0; fr.j = j; fr.addr = best_key & 0xffffffu; fr.score = best;
                     fr.crc = 0;
@@ -402,10 +402,10 @@ __device__ unsigned long long g_solo_t[8];
 #define SOLO_T(i) do { } while (0)
 #endif
 
-// COMPACT (the one-receiver kernel): the capacity check of icao_capacity_kernel is made here, by the CTA itself, while the other
-// threads already fetch the tables; *n_frames_out (shared memory) receives the receiver's frame count, or ~0 when stage B must not run.
+// COMPACT (the one-receiver kernel): the capacity check (capacity_check_all) is made here, by the CTA itself, while the other
+// threads already fetch the tables.  *n_frames_out (shared memory) receives the receiver's frame count, or ~0 when stage B must not run.
 template <bool BIG, bool COMPACT>
-__device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSmem &S, StreamState *st, uint32_t stream, uint32_t *n_frames_out = nullptr) {
+__device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSmem &S, StreamState *st, uint32_t stream, uint32_t *n_frames_out) {
     __shared__ uint32_t s_active, s_gcount[2], s_bits, s_go;
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint32_t LOG2 = BIG ? st->cap_log2 : (uint32_t)ICAO_CAP_LOG2, CAP = 1u << LOG2;
@@ -420,7 +420,7 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
             const uint32_t add = P.stream_addable[stream];
             P.stream_addable[stream] = 0;
             if (P.ctl->overflow & RUN_REPEAT_BITS) go = 0;
-            if (P.prev_ctl && (P.prev_ctl->overflow & RUN_REPEAT_BITS)) { atomicOr(&P.ctl->overflow, 16u); go = 0; }
+            if (P.prev_stop && *P.prev_stop) { atomicOr(&P.ctl->overflow, 16u); go = 0; }
             const uint32_t need = max(g0, g1) + add;
             if (go && 2u * need > CAP) {
                 uint32_t lg = LOG2 + 1;
@@ -429,6 +429,7 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
                 atomicOr(&P.ctl->overflow, 8u);
                 go = 0;
             }
+            *P.stop_out = go ? 0u : 1u;
             if (!go) *n_frames_out = ~0u;
         }
         s_go = go;
@@ -633,8 +634,7 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
             for (int p = 0; p < 5; p++) { atomicAdd(STAT_AT(demod_preamblePhase) + p, (unsigned long long)tot[5 + p]); atomicAdd(STAT_AT(demod_bestPhase) + p, (unsigned long long)tot[10 + p]); }
             atomicAdd(STAT_AT(buffers), (unsigned long long)c_bufs); atomicAdd(STAT_AT(icao_flips), (unsigned long long)c_flips);
 #undef STAT_AT
-            P.frame_count[stream] = min(nframes, P.frame_cap);
-            if (COMPACT) *n_frames_out = min(nframes, P.frame_cap);
+            *n_frames_out = min(nframes, P.frame_cap);
         }
     }
 }
@@ -645,7 +645,57 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
 // changed the filter's membership: then its adds are applied and its frames moved into place.  Otherwise it is resolved
 // again, directly, with the filter as the reference would have it at that point.  In steady state (aircraft already
 // known, no flip) every speculation holds; the results are the sequential ones by construction either way.
-__device__ __forceinline__ void finalize_frames(const FinalizeParams &P, uint32_t warp_global, uint32_t n_warps, uint32_t lane);
+// When its receiver is resolved, the CTA reserves the receiver's range of the packed frame list and finalizes the frames into it.
+__device__ __forceinline__ void finalize_stream(const FinalizeParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane);
+
+// The capacity check of a run, for every receiver (the threads of one CTA share them): (1) the asynchronous pipeline's "the step
+// ahead has to be repeated" test; (2) the filter tables.  stream_addable[s] (scan kernel) bounds the insertions of this run; a
+// generation never exceeds (active now + that), so with 2 x that <= slots no table can fill up and stage B needs no overflow path.
+// A receiver that could exceed it gets grow_log2 set: the host grows its tables and repeats.
+__device__ __forceinline__ void capacity_check_all(const ResolveParams &P) {
+    if (threadIdx.x == 0 && P.prev_stop && *P.prev_stop) atomicOr(&P.ctl->overflow, 16u);
+    for (uint32_t s = threadIdx.x; s < P.n_streams; s += blockDim.x) {
+        const uint32_t add = P.stream_addable[s];
+        P.stream_addable[s] = 0;
+        StreamState *st = &P.state[s];
+        const uint32_t need = max(st->gen_count[0], st->gen_count[1]) + add;
+        if (2u * need > (1u << st->cap_log2)) {
+            uint32_t lg = st->cap_log2 + 1;
+            while ((1u << lg) < 4u * need && lg < ICAO_MAXBITS + 1) lg++;
+            st->grow_log2 = lg;
+            atomicOr(&P.ctl->overflow, 8u);
+        }
+    }
+}
+
+// Whether stage B runs in this run: for no receiver if one of them fails the capacity check, so the check is made ONCE per run,
+// before any CTA touches a receiver's state, by the CTA that claims it first; the other CTAs wait for its verdict.  A CTA only ever
+// waits for a CTA that is already running and needs nothing from the others to finish the check.  The launch for grown tables
+// (a second launch of the same run) finds the verdict made.
+__device__ __forceinline__ bool stage_b_runs(const ResolveParams &P) {
+    __shared__ uint32_t s_verdict;
+    volatile uint32_t *verdict = &P.ctl->cap_check;
+    if (threadIdx.x == 0) s_verdict = atomicCAS(&P.ctl->cap_check, 0u, 1u);
+    __syncthreads();
+    if (s_verdict == 0) {                                 // this CTA claimed the check
+        capacity_check_all(P);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const uint32_t v = (atomicOr(&P.ctl->overflow, 0u) & RUN_REPEAT_BITS) ? CAP_STOP : CAP_GO;
+            *P.stop_out = v == CAP_STOP ? 1u : 0u;
+            __threadfence();
+            *verdict = v;
+            s_verdict = v;
+        }
+    } else if (threadIdx.x == 0) {
+        uint32_t v;
+        while ((v = *verdict) < CAP_STOP) { }
+        __threadfence();
+        s_verdict = v;
+    }
+    __syncthreads();
+    return s_verdict == CAP_GO;
+}
 
 // Receivers with grown tables (BIG) are rare: they get an instantiation of their own, launched only when there is one, so that
 // the common case does not share its register allocation; each CTA of either launch leaves the other kind alone.
@@ -656,14 +706,27 @@ template <bool BIG>
 __global__ void __launch_bounds__(RS_WARPS * 32, RS_MIN_CTAS) resolve_kernel(const ResolveParams P) {
     extern __shared__ uint4 resolve_smem_raw[];
     ResolveSmem &S = *reinterpret_cast<ResolveSmem *>(resolve_smem_raw);
+    __shared__ uint32_t s_nframes, s_base;
     const uint32_t stream = blockIdx.x;
     StreamState *st = &P.state[stream];
-    // Stage A failed (record pool / staging), a receiver's filter tables have to grow first (icao_capacity_kernel), or the step
-    // ahead of this one in the asynchronous pipeline has to be repeated: leave every receiver's state untouched; the host
-    // repairs and repeats the run(s) in order.
-    if (P.ctl->overflow & RUN_REPEAT_BITS) return;
+    // Stage A failed (record pool / staging), a receiver's filter tables have to grow first, or the step ahead of this one in the
+    // asynchronous pipeline has to be repeated: leave every receiver's state untouched, report no frames; the host repairs and
+    // repeats the run(s) in order.
+    if (!stage_b_runs(P)) {
+        if (threadIdx.x == 0) { P.fin.frame_span[2 * stream] = 0; P.fin.frame_span[2 * stream + 1] = 0; }
+        return;
+    }
     if ((st->cap_log2 != ICAO_CAP_LOG2) != BIG) return;
-    resolve_stream<BIG, false>(P, S, st, stream);
+    resolve_stream<BIG, false>(P, S, st, stream, &s_nframes);
+    __syncthreads();
+    // One reservation per receiver: its frames stay together and in order.  Where the receivers' ranges lie relative to each other
+    // depends on which CTA gets here first; frame_span tells every reader where each receiver's frames are.
+    if (threadIdx.x == 0) {
+        s_base = atomicAdd(&P.ctl->total_frames, s_nframes);
+        P.fin.frame_span[2 * stream] = s_base; P.fin.frame_span[2 * stream + 1] = s_nframes;
+    }
+    __syncthreads();
+    finalize_stream(P.fin, stream, s_base, s_nframes, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
 }
 
 __device__ __noinline__ void resolve_stream_big(const ResolveParams &P, ResolveSmem &S, StreamState *st, uint32_t stream, uint32_t *n_frames_out) { resolve_stream<true, true>(P, S, st, stream, n_frames_out); }
@@ -684,12 +747,12 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
     else resolve_stream_big(P, S, st, stream, &s_nframes);
     __syncthreads();
     const uint32_t n = s_nframes == ~0u ? 0u : s_nframes;         // ~0: stage B did not run (the step is going to be repeated)
-    if (threadIdx.x == 0) { P.fin.frame_prefix_out[0] = 0; P.fin.frame_prefix_out[1] = n; P.ctl->total_frames = n; }
-    __syncthreads();
+    if (threadIdx.x == 0) { P.fin.frame_span[0] = 0; P.fin.frame_span[1] = n; P.ctl->total_frames = n; }
 #ifdef B200_SOLO_CLOCKS
+    __syncthreads();
     if (threadIdx.x == 0) g_solo_t[4] = gtime();
 #endif
-    finalize_frames(P.fin, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
+    finalize_stream(P.fin, stream, 0, n, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
     if (P.carry_src && s_nframes != ~0u) {      // (not when the step is going to be repeated: it needs its halo again) every reader of this
                                                 // run's samples - scan kernel, finalizer above - is done: move the tail to the front
         __syncthreads();
@@ -714,31 +777,10 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
 #endif
 }
 
-// Runs ahead of resolve_kernel on its stream: (1) the asynchronous pipeline's "the step ahead has to be repeated" test, once
-// for the whole grid; (2) the capacity check of the receivers' filter tables.  stream_addable[s] (scan kernel) bounds the
-// insertions of this run; a generation never exceeds (active now + that), so with 2 x that <= slots no table can fill up and
-// stage B needs no overflow path.  A receiver that could exceed it gets grow_log2 set: the host grows its tables and repeats.
-__global__ void icao_capacity_kernel(StreamState *state, uint32_t *stream_addable, uint32_t n_streams, RunCtl *ctl, const RunCtl *prev_ctl) {
-    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s == 0 && prev_ctl && (prev_ctl->overflow & RUN_REPEAT_BITS)) atomicOr(&ctl->overflow, 16u);
-    if (s >= n_streams) return;
-    const uint32_t add = stream_addable[s];
-    stream_addable[s] = 0;
-    StreamState *st = &state[s];
-    const uint32_t need = max(st->gen_count[0], st->gen_count[1]) + add;
-    if (2u * need > (1u << st->cap_log2)) {
-        uint32_t lg = st->cap_log2 + 1;
-        while ((1u << lg) < 4u * need && lg < ICAO_MAXBITS + 1) lg++;
-        st->grow_log2 = lg;
-        atomicOr(&ctl->overflow, 8u);
-    }
-}
-
 // ------------------------------------------------------------------------------------------------
+// Mode A/C: exclusive prefix of the per-buffer reply counts (ac_pack_kernel packs the lists with it)
 // ------------------------------------------------------------------------------------------------
-// finalize: prefix of per-stream frame counts, then one warp per frame
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) frame_prefix_kernel(const uint32_t *count, uint32_t *prefix, uint32_t n, RunCtl *ctl, bool set_total = true) {
+__global__ void __launch_bounds__(1024) frame_prefix_kernel(const uint32_t *count, uint32_t *prefix, uint32_t n, const RunCtl *ctl) {
     const uint32_t n_all = n;
     __shared__ uint32_t scratch[40];
     uint32_t base = 0;
@@ -752,27 +794,16 @@ __global__ void __launch_bounds__(1024) frame_prefix_kernel(const uint32_t *coun
         base += total;
     }
     for (uint32_t i = n + threadIdx.x; i < n_all; i += blockDim.x) prefix[i] = base;
-    if (threadIdx.x == 0) { prefix[n_all] = base; if (set_total) ctl->total_frames = base; }
+    if (threadIdx.x == 0) prefix[n_all] = base;
 }
 
 __device__ __forceinline__ unsigned long long dmax_bits(double v) { return (unsigned long long)__double_as_longlong(v); }
 
-// One warp per accepted frame: the frame from its record, its signal power, the statistics (see the file header).  `warp_global` of
-// `n_warps` warps share the frames of the run.
-__device__ __forceinline__ void finalize_frames(const FinalizeParams &P, uint32_t warp_global, uint32_t n_warps, uint32_t lane) {
-    const uint32_t total = P.frame_prefix[P.n_streams];
-    for (uint32_t fi = warp_global; fi < total; fi += n_warps) {
-        // stream = last s with prefix[s] <= fi.  The whole kernel is one dependent-load chain per frame, so the search is done by
-        // the warp, 32 probes per level (two loads deep for 256 receivers instead of eight), ...
-        uint32_t lo = 0, span = P.n_streams;                     // the answer lies in [lo, lo + span)
-        while (span > 1) {
-            const uint32_t step = (span + 31) >> 5, idx = lo + lane * step;
-            const bool le = lane * step < span && P.frame_prefix[idx] <= fi;          // true for lane 0: prefix[lo] <= fi
-            const uint32_t j = __popc(__ballot_sync(FULLMASK, le)) - 1u;              // prefixes ascend: the true lanes are 0..j
-            lo += j * step;
-            span = min(step, span - j * step);
-        }
-        const uint32_t stream = lo, k = fi - P.frame_prefix[lo];
+// One warp per accepted frame of receiver `stream`: the frame from its record, its signal power, the statistics (see the file
+// header).  Warp `warp` of `n_warps` takes frames warp, warp + n_warps, ... of the receiver's n and writes frame k to packed[base + k].
+__device__ __forceinline__ void finalize_stream(const FinalizeParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane) {
+    for (uint32_t k = warp; k < n; k += n_warps) {
+        const uint32_t fi = base + k;
         const b200_frame *src = &P.frames[(size_t)stream * P.frame_cap + k];
         const uint32_t d = *reinterpret_cast<const uint32_t *>(&src->pad_[2]);
         // locate the segment: accept records carry the low 16 bits of the segment index; a stream has few segments
@@ -783,7 +814,7 @@ __device__ __forceinline__ void finalize_frames(const FinalizeParams &P, uint32_
         }
         const Segment seg = P.one_seg_valid ? P.one_seg : P.segs[seg_i];
         const uint32_t len = src->signal_len;                    // 134 or 268 samples (demod_2400.c:439): at most 9 per lane
-        // ... and the samples are fetched with all loads of a lane in flight at once (then the table lookups, likewise)
+        // the samples are fetched with all loads of a lane in flight at once (then the table lookups, likewise)
         constexpr int FIN_PER_LANE = 9;
         uint32_t raw[FIN_PER_LANE];
 #pragma unroll
@@ -844,11 +875,6 @@ __device__ __forceinline__ void finalize_frames(const FinalizeParams &P, uint32_
             atomicMax((unsigned long long *)&s.peak_signal_power, dmax_bits(level));
         }
     }
-}
-
-// Small CTAs (128 threads x 48 registers): they have to fit into what the persistent scan kernel of the NEXT step leaves free on an SM.
-__global__ void __launch_bounds__(128) finalize_kernel(const FinalizeParams P) {
-    finalize_frames(P, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, threadIdx.x & 31);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -936,19 +962,12 @@ extern "C" int b200_prepare_resolve(void) {      // per device, from b200_demod_
 
 // any_grown: some receiver of the context has filter tables of its own (then the second instantiation runs too; returns the launches made)
 extern "C" int b200_launch_resolve(const ResolveParams *p, int any_grown, void *stream) {
-    if (p->solo) {          // one receiver: capacity check, stage B, frame prefix and finalizer in one launch
+    if (p->solo) {          // one receiver: capacity check, stage B, frame placement and finalizer in one launch
         resolve_solo_kernel<<<1, RS_WARPS * 32, sizeof(ResolveSmem), (cudaStream_t)stream>>>(*p);
         return (int)cudaGetLastError();
     }
-    icao_capacity_kernel<<<(p->n_streams + 127) / 128, 128, 0, (cudaStream_t)stream>>>(p->state, p->stream_addable, p->n_streams, p->ctl, p->prev_ctl);
     resolve_kernel<false><<<p->n_streams, RS_WARPS * 32, sizeof(ResolveSmem), (cudaStream_t)stream>>>(*p);
     if (any_grown) resolve_kernel<true><<<p->n_streams, RS_WARPS * 32, sizeof(ResolveSmem), (cudaStream_t)stream>>>(*p);
-    return (int)cudaGetLastError();
-}
-
-extern "C" int b200_launch_finalize(const FinalizeParams *p, uint32_t *d_frame_prefix, RunCtl *ctl, int n_sm, void *stream) {
-    frame_prefix_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(p->frame_count, d_frame_prefix, p->n_streams, ctl);
-    finalize_kernel<<<n_sm * 4, 128, 0, (cudaStream_t)stream>>>(*p);
     return (int)cudaGetLastError();
 }
 
@@ -962,7 +981,7 @@ extern "C" int b200_launch_icao_rehash(StreamState *state, uint32_t stream, uint
     return (int)cudaGetLastError();
 }
 
-// Mode A/C: pack the per-buffer reply lists in buffer order (prefix by the frame prefix kernel, then one block per buffer).
+// Mode A/C: pack the per-buffer reply lists in buffer order (prefix by frame_prefix_kernel, then one block per buffer).
 __global__ void ac_pack_kernel(const b200_modeac *ac_out, const uint32_t *count, const uint32_t *prefix, b200_modeac *packed, uint32_t cap, const RunCtl *ctl) {
     if (ctl->overflow & RUN_REPEAT_BITS) return;          // the walk did not run (this step is going to be repeated): its counts are not this run's
     const uint32_t s = blockIdx.x;
@@ -972,7 +991,7 @@ __global__ void ac_pack_kernel(const b200_modeac *ac_out, const uint32_t *count,
 
 extern "C" int b200_launch_ac_pack(const b200_modeac *ac_out, const uint32_t *count, uint32_t *prefix, b200_modeac *packed, uint32_t n_units,
                                    uint32_t cap, RunCtl *ctl, void *stream) {
-    frame_prefix_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(count, prefix, n_units, ctl, false);
+    frame_prefix_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(count, prefix, n_units, ctl);
     if (n_units) ac_pack_kernel<<<n_units, 32, 0, (cudaStream_t)stream>>>(ac_out, count, prefix, packed, cap, ctl);
     return (int)cudaGetLastError();
 }
