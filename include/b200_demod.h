@@ -240,6 +240,28 @@ int b200_demod_run_host_uc8_async(b200_demod_ctx *ctx, const uint8_t *h_iq, uint
                                   uint32_t n_buffers, uint32_t buf_len, int continues,
                                   int64_t first_sample_timestamp);
 
+/* The three calls above for 16-bit frontends (INPUT_SC16: Pluto, SoapySDR devices such as Airspy and SDRplay; INPUT_SC16Q11:
+ * bladeRF), argument for argument, plus q11 as in b200_demod_submit_iq_sc16 (0: convert_sc16_nodc, I / 32768; nonzero:
+ * convert_sc16q11_nodc, I / 2048).  Each receiver's samples are interleaved little-endian int16 I,Q pairs, 4 bytes per sample,
+ * so stream_stride_bytes / host_stride_bytes must be at least n_buffers * buf_len * 4; d_iq and stream_stride_bytes 16-byte
+ * aligned and buf_len a multiple of 8, as for uc8.  continues != 0 means: device path, the 326 samples (1304 bytes) before each
+ * receiver's first sample are valid halo; host path, the previous run_host_sc16_async step's last 326 samples become the halo
+ * (a previous run_host_uc8_async step does not count: B200_E_STATE).
+ * One converter launch per step turns every receiver's halo and buffers into magnitudes, bit for bit the reference's, in a
+ * library-owned slab (allocated on the first such step), ahead of the scan on the same stream; a repeated step converts again.
+ * b200_buffer_result.sum_level / sum_power hold the IEEE-754 bit patterns of the reference's two float sums of each buffer, as for
+ * submit_iq_sc16; with B200_CFG_MODE_AC they give the Mode A/C noise floor.  Steps of both formats share the three pipeline
+ * slots, b200_demod_wait and the fetch calls. */
+int b200_demod_run_device_sc16(b200_demod_ctx *ctx, const int16_t *d_iq, uint64_t stream_stride_bytes,
+                               uint32_t n_buffers, uint32_t buf_len, int continues,
+                               int64_t first_sample_timestamp, int q11);
+int b200_demod_run_device_sc16_async(b200_demod_ctx *ctx, const int16_t *d_iq, uint64_t stream_stride_bytes,
+                                     uint32_t n_buffers, uint32_t buf_len, int continues,
+                                     int64_t first_sample_timestamp, int q11);
+int b200_demod_run_host_sc16_async(b200_demod_ctx *ctx, const int16_t *h_iq, uint64_t host_stride_bytes,
+                                   uint32_t n_buffers, uint32_t buf_len, int continues,
+                                   int64_t first_sample_timestamp, int q11);
+
 /* results of the last run ---------------------------------------------------------------------- */
 int b200_demod_frame_count(b200_demod_ctx *ctx, uint32_t stream, uint32_t *n);
 int b200_demod_fetch(b200_demod_ctx *ctx, uint32_t stream, b200_frame *out, uint32_t cap, uint32_t *n);
@@ -273,7 +295,7 @@ int b200_demod_icao_expire(b200_demod_ctx *ctx, uint32_t stream);
 int b200_demod_icao_reset(b200_demod_ctx *ctx, uint32_t stream);
 
 /* instrumentation: device time (ms) of the last run, by CUDA events on the library's stream:
- * [0] whole run, [1] scan kernel (stage A), [2] resolve kernel (stage B), [3] H2D, [4] D2H.
+ * [0] whole run, [1] scan kernel (stage A; in an sc16 step the converter and the scan), [2] resolve kernel (stage B), [3] H2D, [4] D2H.
  * kernel_launches = number of the library's own kernel launches in the last run. */
 int b200_demod_last_timing(b200_demod_ctx *ctx, float ms[5], uint32_t *kernel_launches);
 

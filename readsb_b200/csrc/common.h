@@ -86,7 +86,7 @@ struct BufAcc {        // exact per-buffer sums (convert.c:75-79), zeroed at the
     unsigned long long sum_level;
     unsigned long long sum_power;
     unsigned long long sum_signal_power;
-    unsigned long long pad_;
+    float2 fsum;       // sc16 steps: the converter's float sums (sum_level, sum_power), written by sc16_convert_kernel
 };
 
 // ---- per-receiver persistent state (device) -----------------------------------------------------
@@ -262,6 +262,18 @@ struct AcWalkParams {
     RunCtl *ctl;
 };
 
+// ---- sc16 / sc16q11 input (convert_kernel.cu) ----------------------------------------------------
+// Buffer g = s * n_buffers + b of a step: receiver s, its buffer b.  Samples are interleaved int16 I,Q (one 32-bit word each).
+struct Sc16Params {
+    const uint32_t *iq;               // receiver s's first new sample at iq + s * iq_stride; with `halo` its 326 raw halo samples precede it
+    uint16_t *mag;                    // receiver s's data index 0 (first halo magnitude) at mag + s * mag_stride
+    float2 *sums;                     // buffer g's float sums (sum_level, sum_power) at sums[g * sums_stride]
+    uint64_t iq_stride, mag_stride;   // in samples
+    uint32_t sums_stride, n_streams, n_buffers, buf_len;
+    uint32_t halo;                    // also convert the halo (the step continues its receivers)
+    float scale;                      // 1 / 32768 (sc16) or 1 / 2048 (sc16q11)
+};
+
 struct BeastParams {                 // beast_kernel.cu
     const Segment *segs;
     const uint32_t *stream_seg_begin;
@@ -301,7 +313,8 @@ int b200_launch_resolve(const ResolveParams *p, int any_grown, void *stream);
 int b200_launch_init_state(StreamState *state, uint32_t n, uint32_t *slab, void *stream);
 int b200_launch_icao_rehash(StreamState *state, uint32_t stream, uint32_t *new0, uint32_t *new1, uint32_t new_log2, void *stream_);
 int b200_launch_modeac(const AcScanParams *sp, const AcWalkParams *wp, int n_sm, void *stream);
-int b200_launch_sc16_convert(const void *d_iq, uint16_t *d_mag, uint32_t n, int q11, float2 *d_sums, int n_sm, void *stream);
+int b200_prepare_convert(void);
+int b200_launch_sc16_convert(const Sc16Params *p, void *stream);
 int b200_launch_beast(const BeastParams *p, uint32_t n_streams, void *stream);
 int b200_launch_modeac_stats(const AcWalkParams *wp, const uint32_t *prefix, void *stream);
 int b200_launch_ac_pack(const b200_modeac *ac_out, const uint32_t *count, uint32_t *prefix, b200_modeac *packed, uint32_t n_units, uint32_t cap, RunCtl *ctl, void *stream);

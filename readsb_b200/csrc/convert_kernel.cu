@@ -1,17 +1,32 @@
 // convert_kernel.cu — the float-path IQ converters (SURVEY.md section 8f row 3): convert_sc16_nodc convert.c:212-250 and
 // convert_sc16q11_nodc convert.c:329-367 (the default build has no SC16Q11 table), for bladeRF / Pluto / Soapy style input.
 //
-//   sc16_mag_kernel   data parallel: int16 I, Q -> uint16 magnitude, exactly the reference's float expression
-//                     (I / 32768 or I / 2048 is an exact scaling, the two products and their sum are rounded separately —
-//                     the library is built with --fmad=false —, sqrtf is correctly rounded, * 65535 + 0.5 are two operations)
-//   sc16_sum_kernel   the reference also returns mean_level / mean_power from FLOAT accumulators that are added to in
-//                     sample order (convert.c:225,238-239); a float sum is not associative, so one warp per buffer keeps the
-//                     order: the lanes compute 32 samples' magnitude / power in parallel, then every lane adds the 32 values
-//                     in sample order (shuffles), all lanes holding the same running sums.
+// One launch converts a whole step: every receiver's buffers (and, for a continued receiver, its 326-sample halo) into
+// uint16 magnitudes, and every buffer's two float sums.
 //
-// The magnitudes go into the receiver's arena like a magnitude hand-off, and the Mode S pipeline runs on them unchanged.
+//   magnitudes   exactly the reference's float expression (I / 32768 or I / 2048 is an exact scaling, the two products and
+//                their sum are rounded separately — the library is built with --fmad=false —, sqrtf is correctly rounded,
+//                * 65535 + 0.5 are two operations).  A pure function of the sample, so a halo converted again from the raw
+//                halo equals the magnitudes the previous step made of the same samples.
+//   sums         the reference returns mean_level / mean_power of these formats from FLOAT accumulators added to in sample
+//                order (convert.c:225,238-239).  A float sum is not associative, so each buffer's two sums are two dependent
+//                chains of adds in sample order; a parallel reduction would give other bits.
+//
+// A CTA owns SC16_GROUP buffers of equal length and walks them in blocks of SC16_BLOCK samples.  Its eight worker warps
+// convert block k data parallel (coalesced 4-byte loads and 2-byte stores; the loads of block k+1 are issued before block k
+// is converted) and stage each sample's float mag / magsq in shared memory; meanwhile lane 2j / 2j+1 of the ninth warp adds
+// block k-1's staged values of buffer j to its level / power sum.  One warp instruction thus advances 32 chains, and the
+// chains of all buffers of a step run at the same time: the step pays one chain of buf_len dependent adds (about
+// 4 cycles each), not one per buffer.
 #include "common.h"
 #include "device_utils.cuh"
+
+#define SC16_GROUP   16                          // buffers per CTA: two chains each in the summing warp
+#define SC16_BLOCK   512                         // samples per buffer and block
+#define SC16_ROW     (SC16_BLOCK + 4)            // staged floats per chain: +4 keeps the summing warp's 16-byte reads conflict-free
+#define SC16_WORKERS 256
+#define SC16_PER_THREAD (SC16_GROUP * SC16_BLOCK / SC16_WORKERS)
+#define SC16_SMEM    (2 * 2 * SC16_GROUP * SC16_ROW * (int)sizeof(float))    // two blocks in turn
 
 __device__ __forceinline__ void sc16_sample(uint32_t iq, float scale, float &mag, float &magsq) {
     const float fI = (float)(int16_t)(iq & 0xffffu) * scale, fQ = (float)(int16_t)(iq >> 16) * scale;   // I / 32768.0f resp. I / 2048.0f: exact
@@ -21,38 +36,98 @@ __device__ __forceinline__ void sc16_sample(uint32_t iq, float scale, float &mag
     mag = sqrtf(magsq);
 }
 
-__global__ void __launch_bounds__(256) sc16_mag_kernel(const uint32_t *__restrict__ iq, uint16_t *__restrict__ mag_out, uint32_t n, float scale) {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        float mag, magsq;
-        sc16_sample(iq[i], scale, mag, magsq);
-        const float scaled = mag * 65535.0f;
-        mag_out[i] = (uint16_t)(scaled + 0.5f);
-    }
+__device__ __forceinline__ uint16_t sc16_mag_u16(float mag) {
+    const float scaled = mag * 65535.0f;
+    return (uint16_t)(scaled + 0.5f);
 }
 
-__global__ void __launch_bounds__(32) sc16_sum_kernel(const uint32_t *__restrict__ iq, uint32_t n, float scale, float2 *out) {
-    const uint32_t lane = threadIdx.x;
-    float sum_level = 0.0f, sum_power = 0.0f;
-    for (uint32_t i0 = 0; i0 < n; i0 += 32) {
-        float mag = 0.0f, magsq = 0.0f;
-        if (i0 + lane < n) sc16_sample(iq[i0 + lane], scale, mag, magsq);
-        const uint32_t cnt = min(32u, n - i0);
-        if (cnt == 32) {
-#pragma unroll
-            for (int k = 0; k < 32; k++) { sum_power += __shfl_sync(FULLMASK, magsq, k); sum_level += __shfl_sync(FULLMASK, mag, k); }
-        } else {
-            for (uint32_t k = 0; k < cnt; k++) { sum_power += __shfl_sync(FULLMASK, magsq, k); sum_level += __shfl_sync(FULLMASK, mag, k); }
+__global__ void __launch_bounds__(SC16_WORKERS + 32, 1) sc16_convert_kernel(const Sc16Params P) {
+    extern __shared__ __align__(16) float sc16_stage[];       // [2][2 * SC16_GROUP][SC16_ROW]
+    const uint32_t tid = threadIdx.x;
+    const uint32_t nbuf = P.n_streams * P.n_buffers, g0 = blockIdx.x * SC16_GROUP;
+    const uint32_t n_here = min((uint32_t)SC16_GROUP, nbuf - g0);
+
+    // halos of the receivers whose first buffer is in this CTA: converted, not summed
+    if (P.halo) {
+        for (uint32_t s = (g0 + P.n_buffers - 1) / P.n_buffers; s * P.n_buffers < g0 + n_here; s++) {
+            const uint32_t *in = P.iq + s * P.iq_stride - B200_TRAIL;
+            uint16_t *out = P.mag + s * P.mag_stride;
+            for (uint32_t i = tid; i < B200_TRAIL; i += blockDim.x) {
+                float mag, magsq;
+                sc16_sample(in[i], P.scale, mag, magsq);
+                out[i] = sc16_mag_u16(mag);
+            }
         }
     }
-    if (lane == 0) *out = make_float2(sum_level, sum_power);
+
+    const uint32_t n_blocks = (P.buf_len + SC16_BLOCK - 1) / SC16_BLOCK;
+    if (tid < SC16_WORKERS) {
+        // item r of this thread: buffer r / 2 of the group, sample tid + 256 * (r & 1) of the block
+        const uint32_t *src[SC16_GROUP];
+        uint16_t *dst[SC16_GROUP];
+#pragma unroll
+        for (int j = 0; j < SC16_GROUP; j++) {
+            const uint32_t g = g0 + min((uint32_t)j, n_here - 1), s = g / P.n_buffers, b = g % P.n_buffers;
+            src[j] = P.iq + s * P.iq_stride + (size_t)b * P.buf_len;
+            dst[j] = P.mag + s * P.mag_stride + B200_TRAIL + (size_t)b * P.buf_len;
+        }
+        uint32_t nxt[SC16_PER_THREAD];
+        auto load = [&](uint32_t k) {
+#pragma unroll
+            for (int r = 0; r < SC16_PER_THREAD; r++) {
+                const uint32_t i = k * SC16_BLOCK + tid + SC16_WORKERS * (r & 1);
+                nxt[r] = ((uint32_t)(r >> 1) < n_here && i < P.buf_len) ? __ldg(src[r >> 1] + i) : 0u;
+            }
+        };
+        load(0);
+        for (uint32_t k = 0; k <= n_blocks; k++) {
+            if (k < n_blocks) {
+                uint32_t cur[SC16_PER_THREAD];
+#pragma unroll
+                for (int r = 0; r < SC16_PER_THREAD; r++) cur[r] = nxt[r];
+                if (k + 1 < n_blocks) load(k + 1);
+                float *stage = sc16_stage + (k & 1) * (2 * SC16_GROUP * SC16_ROW);
+#pragma unroll
+                for (int r = 0; r < SC16_PER_THREAD; r++) {
+                    // every item, also of absent buffers: a guard between the items costs the full groups more than it saves
+                    const uint32_t x = tid + SC16_WORKERS * (r & 1), i = k * SC16_BLOCK + x;
+                    float mag, magsq;
+                    sc16_sample(cur[r], P.scale, mag, magsq);       // a missing sample is (0, 0): 0 + 0.0f leaves a sum as it is
+                    if ((uint32_t)(r >> 1) < n_here && i < P.buf_len) dst[r >> 1][i] = sc16_mag_u16(mag);
+                    stage[(2 * (r >> 1)) * SC16_ROW + x] = mag;
+                    stage[(2 * (r >> 1) + 1) * SC16_ROW + x] = magsq;
+                }
+            }
+            __syncthreads();
+        }
+    } else {
+        const uint32_t lane = tid - SC16_WORKERS;            // chain: buffer lane / 2, level (even lane) or power (odd lane)
+        float sum = 0.0f;
+        for (uint32_t k = 0; k <= n_blocks; k++) {
+            if (k > 0) {
+                const float4 *row = reinterpret_cast<const float4 *>(sc16_stage + ((k - 1) & 1) * (2 * SC16_GROUP * SC16_ROW) + lane * SC16_ROW);
+#pragma unroll 16
+                for (int q = 0; q < SC16_BLOCK / 4; q++) {
+                    const float4 v = row[q];
+                    sum += v.x; sum += v.y; sum += v.z; sum += v.w;
+                }
+            }
+            __syncthreads();
+        }
+        if (lane / 2 < n_here) {
+            float *out = reinterpret_cast<float *>(P.sums + (size_t)(g0 + lane / 2) * P.sums_stride);
+            out[lane & 1] = sum;
+        }
+    }
 }
 
-extern "C" int b200_launch_sc16_convert(const void *d_iq, uint16_t *d_mag, uint32_t n, int q11, float2 *d_sums, int n_sm, void *stream) {
-    if (!n) return 0;
-    const float scale = q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
-    uint32_t grid = (n + 255) / 256;
-    if (grid > (uint32_t)n_sm * 4) grid = (uint32_t)n_sm * 4;
-    sc16_mag_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t *>(d_iq), d_mag, n, scale);
-    sc16_sum_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t *>(d_iq), n, scale, d_sums);
+extern "C" int b200_prepare_convert(void) {      // per device, from b200_demod_create
+    return (int)cudaFuncSetAttribute(sc16_convert_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SC16_SMEM);
+}
+
+extern "C" int b200_launch_sc16_convert(const Sc16Params *p, void *stream) {
+    const uint32_t nbuf = p->n_streams * p->n_buffers;
+    if (!nbuf || !p->buf_len) return 0;
+    sc16_convert_kernel<<<(nbuf + SC16_GROUP - 1) / SC16_GROUP, SC16_WORKERS + 32, SC16_SMEM, (cudaStream_t)stream>>>(*p);
     return (int)cudaGetLastError();
 }

@@ -6,7 +6,7 @@
 // demodulate2400(buf) (readsb.c:871, demod_2400.h:38) becomes submit_mag_u16 / run / fetch.
 //
 // A run owns one SLOT (segment tables, candidate pools, result buffers).  The blocking calls use slot 0 on one
-// CUDA stream.  The asynchronous calls (run_device_uc8_async / run_host_uc8_async / wait) cycle through NSLOT slots: the
+// CUDA stream.  The asynchronous calls (run_device_*_async / run_host_*_async / wait) cycle through NSLOT slots: the
 // scan kernels of consecutive steps run back to back on the scan stream, stage B (one launch: capacity check, stage B, frame
 // placement, finalizer) + D2H of each step follow on the resolve stream (higher priority) as soon as its scan has ended; stage B
 // kernels stay ordered among themselves, which is all the per-receiver state needs.
@@ -37,8 +37,12 @@ struct Pending {
     double mean_level = 0, mean_power = 0;
 };
 
+// sample format of a device-resident or pipelined step
+enum IqFormat { FMT_UC8 = 0, FMT_SC16 = 1, FMT_SC16Q11 = 2 };
+static inline uint32_t fmt_bytes(int fmt) { return fmt == FMT_UC8 ? 2u : 4u; }     // bytes per raw sample
+
 struct DeviceArgs {      // what a device-resident step was asked to do (kept for a repeat after a pool regrowth)
-    const uint8_t *d_iq; uint64_t stride; uint32_t n_buffers, buf_len; int continues; int64_t first_ts;
+    const uint8_t *d_iq; uint64_t stride; uint32_t n_buffers, buf_len; int continues; int64_t first_ts; int fmt;
 };
 
 struct Slot {
@@ -88,6 +92,12 @@ struct Slot {
     bool desc_on_device = true;       // false: this run's descriptors went as kernel parameters (b200_demod_fetch_beast uploads them if asked)
     int scan_grid = 0;                // CTAs the scan kernel of this run was launched with
     bool published = false, timed = true;   // this run: results published by the kernel / events recorded between the kernels
+    // sc16 / sc16q11 steps: the run's magnitudes, made by sc16_convert_kernel on the scan stream ahead of the scan (again when the
+    // step is repeated); its float sums go to BufAcc::fsum of the run's buffers and come back with the result block
+    bool sc16 = false;
+    Sc16Params conv = {};
+    uint16_t *d_slab = nullptr;       // receiver s at d_slab + s * slab_stride: 2 samples of padding (new samples 16-byte aligned),
+    size_t slab_stride = 0;           // 326 halo magnitudes, max_buffers_per_run * buf_samples magnitudes; allocated on the first sc16 step
 };
 
 #define FIRST_COPY_FRAMES 16
@@ -158,9 +168,12 @@ struct b200_demod_ctx {
     // pipelined host-buffer path (run_host_uc8_async): two device input buffers, one per pipeline slot, filled on in_stream
     uint8_t *d_pipe[NSLOT] = {};
     size_t pipe_stride = 0;
+    uint8_t *d_pipe16[NSLOT] = {};    // ... the same for run_host_sc16_async (int16 samples), allocated on its first step
+    size_t pipe16_stride = 0;
     cudaEvent_t ev_in[NSLOT] = {};
     bool pipe_prev_valid = false;     // the buffer of the previous step holds >= 326 samples per receiver
     int pipe_prev = 0; size_t pipe_prev_row = 0;
+    uint32_t pipe_prev_bytes = 0;     // bytes per sample of the previous step (2 uc8, 4 sc16): a halo only continues the same input width
 };
 
 static int fail(b200_demod_ctx *c, int code, const char *fmt, ...) {
@@ -226,6 +239,7 @@ static void free_slot(Slot &s) {
     cudaFree(s.d_mag_copy); cudaFree(s.d_ac_bitmap); cudaFree(s.d_ac_noise); cudaFree(s.d_ac_count); cudaFree(s.d_ac_prefix); cudaFree(s.d_ac_out); cudaFree(s.d_ac_packed);
     cudaFreeHost(s.h_ac_prefix); cudaFreeHost(s.h_ac_packed);
     cudaFree(s.d_ac_levels); cudaFreeHost(s.h_ac_levels);
+    cudaFree(s.d_slab);
     free(s.h_segs); free(s.h_tile_seg); free(s.h_stream_seg_begin);
     for (auto &e : s.ev) if (e) cudaEventDestroy(e);
     s = Slot();
@@ -313,7 +327,7 @@ API void b200_demod_destroy(b200_demod_ctx *c) {
     if (c->res_stream) cudaStreamDestroy(c->res_stream);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->in_stream) cudaStreamDestroy(c->in_stream);
-    for (int i = 0; i < NSLOT; i++) { cudaFree(c->d_pipe[i]); if (c->ev_in[i]) cudaEventDestroy(c->ev_in[i]); }
+    for (int i = 0; i < NSLOT; i++) { cudaFree(c->d_pipe[i]); cudaFree(c->d_pipe16[i]); if (c->ev_in[i]) cudaEventDestroy(c->ev_in[i]); }
     delete c;
 }
 
@@ -378,6 +392,7 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
     }
     // kernel attributes (dynamic shared memory opt-in) are per device: set them for this context's device, every time
     CUC((cudaError_t)b200_prepare_scan()); CUC((cudaError_t)b200_prepare_resolve()); CUC((cudaError_t)b200_prepare_modeac());
+    CUC((cudaError_t)b200_prepare_convert());
     CUC(dev_alloc(&c->d_state, S));
     CUC(dev_alloc(&c->d_icao_slab, (size_t)S * 2 * ICAO_CAP));
     CUC((cudaError_t)b200_launch_init_state(c->d_state, S, c->d_icao_slab, c->stream));
@@ -501,9 +516,13 @@ API int b200_demod_submit_iq_sc16(b200_demod_ctx *c, uint32_t s, const int16_t *
     uint8_t *region = c->d_arena + (size_t)s * c->stream_stride;
     Pending p;
     p.n = n; p.ts = ts; p.off = c->cursor[s]; p.fsum = (int)c->n_fsum++;
-    // one staging buffer: the copy and the two kernels of this submit are ordered on the stream before the next submit's copy
+    // one staging buffer: the copy and the converter of this submit are ordered on the stream before the next submit's copy
     if (n) CU(c, cudaMemcpyAsync(c->d_raw16, iq, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
-    { int r = b200_launch_sc16_convert(c->d_raw16, reinterpret_cast<uint16_t *>(region + p.off), n, q11, c->d_fsum + p.fsum, c->n_sm, c->stream);
+    Sc16Params cp = {};
+    cp.iq = reinterpret_cast<const uint32_t *>(c->d_raw16); cp.mag = reinterpret_cast<uint16_t *>(region + p.off) - B200_TRAIL;
+    cp.sums = c->d_fsum + p.fsum; cp.sums_stride = 1; cp.n_streams = 1; cp.n_buffers = 1; cp.buf_len = n;
+    cp.scale = q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
+    { int r = b200_launch_sc16_convert(&cp, c->stream);
       if (r) return fail(c, B200_E_CUDA, "sc16 convert launch: %s", cudaGetErrorString((cudaError_t)r)); }
     c->cursor[s] = p.off + (size_t)n * 2;
     c->pending[s].push_back(p);
@@ -583,6 +602,11 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     sp.long_set = (1u << 16) | (1u << 17) | (1u << 18) | (1u << 20) | (1u << 21);
     if (sp.nfix && sp.fixdf) for (int b = 0; b < 5; b++) sp.long_set |= 1u << (17 ^ (1 << b));
     if (timing) CU(c, cudaEventRecord(sl.ev[0], scan));
+    if (sl.sc16) {          // after the zeroing of the per-buffer sums above: the converter writes BufAcc::fsum
+        sl.conv.sums = &sl.d_buf_acc->fsum; sl.conv.sums_stride = sizeof(BufAcc) / sizeof(float2);
+        int r = b200_launch_sc16_convert(&sl.conv, scan); if (r) return fail(c, B200_E_CUDA, "sc16 convert launch: %s", cudaGetErrorString((cudaError_t)r));
+        sl.launches++;
+    }
     sl.scan_grid = scan != res ? ((c->part_fixed || !c->part_n) ? c->n_sm_scan_async : c->part_n) : c->n_sm_scan;
     if (sl.ntile) { int r = b200_launch_scan(&sp, c->d_tables, sl.scan_grid, scan); if (r) return fail(c, B200_E_CUDA, "scan launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches++; }
     if (timing) CU(c, cudaEventRecord(sl.ev[1], scan));
@@ -595,7 +619,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     if (mode_ac) {
         if (sl.nbuf) CU(c, cudaMemcpyAsync(sl.d_ac_levels, sl.h_ac_levels, (size_t)sl.nbuf * sizeof(AcLevel), cudaMemcpyHostToDevice, scan));
         AcScanParams as;
-        as.levels = sl.d_ac_levels; as.fsum = c->d_fsum;
+        as.levels = sl.d_ac_levels; as.fsum = sl.sc16 ? &sl.d_buf_acc->fsum : c->d_fsum;
         as.segs = sl.d_segs; as.n_segs = sl.nseg; as.tile_seg = sl.d_tile_seg; as.n_tiles = sl.ntile; as.buf_acc = sl.d_buf_acc;
         as.tables = c->d_tables; as.noise = sl.d_ac_noise; as.bitmap = sl.d_ac_bitmap; as.ctl = sl.d_ctl; as.mag_copy = sl.d_mag_copy;
         aw.segs = sl.d_segs; aw.n_segs = sl.nseg; aw.stream_seg_begin = sl.d_stream_seg_begin; aw.n_streams = S; aw.bitmap = sl.d_ac_bitmap;
@@ -684,6 +708,11 @@ static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
         sl.h_buf_out[b].sum_power = sl.h_buf_acc[b].sum_power;
         sl.h_buf_out[b].sum_signal_power = sl.h_buf_acc[b].sum_signal_power;
     }
+    if (sl.sc16) for (uint32_t b = 0; b < sl.nbuf; b++) {     // the reference's float accumulators instead of the integer sums
+        uint32_t lv, pw;
+        memcpy(&lv, &sl.h_buf_acc[b].fsum.x, 4); memcpy(&pw, &sl.h_buf_acc[b].fsum.y, 4);
+        sl.h_buf_out[b].sum_level = lv; sl.h_buf_out[b].sum_power = pw;
+    }
     if (sl.timed) {
         cudaEventElapsedTime(&sl.ms[1], sl.ev[0], sl.ev[1]);
         cudaEventElapsedTime(&sl.ms[2], sl.ev[1], sl.ev[2]);
@@ -764,7 +793,7 @@ API int b200_demod_run(b200_demod_ctx *c) {
     const uint32_t S = c->cfg.n_streams, BUF = c->cfg.buf_samples;
     Slot &sl = c->slot[0];
     c->cur = 0;
-    sl.nseg = sl.ntile = sl.nbuf = 0; sl.is_device = false; sl.upload_tiles = true; sl.cached_tiles = 0;
+    sl.nseg = sl.ntile = sl.nbuf = 0; sl.is_device = false; sl.upload_tiles = true; sl.cached_tiles = 0; sl.sc16 = false;
     std::vector<std::pair<uint32_t, int>> fsum_of_buf;      // (buffer of the run, float-sum slot) for sc16 buffers
     std::vector<std::pair<uint32_t, const Pending *>> given_levels;   // (buffer of the run, hand-off that brought its own mean_level / mean_power)
     std::vector<uint8_t> halo_after(c->halo_valid);        // committed only when the run succeeded (a failed run leaves no halo behind)
@@ -844,38 +873,68 @@ API int b200_demod_run(b200_demod_ctx *c) {
 }
 
 static int build_device_run(b200_demod_ctx *c, Slot &sl, const DeviceArgs &a) {
-    const uint32_t S = c->cfg.n_streams;
+    const uint32_t S = c->cfg.n_streams, bps = fmt_bytes(a.fmt);
     if (((uintptr_t)a.d_iq & 15) || (a.stride & 15) || (a.buf_len & 7)) return fail(c, B200_E_INVAL, "d_iq and stream_stride_bytes must be 16-byte aligned and buf_len a multiple of 8");
     if (a.n_buffers == 0 || a.n_buffers > c->cfg.max_buffers_per_run || a.buf_len == 0 || a.buf_len > c->cfg.buf_samples) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration");
-    if ((uint64_t)a.n_buffers * a.buf_len * 2 > a.stride && S > 1) return fail(c, B200_E_INVAL, "stream_stride_bytes smaller than one stream's data");
+    if ((uint64_t)a.n_buffers * a.buf_len * bps > a.stride && S > 1) return fail(c, B200_E_INVAL, "stream_stride_bytes smaller than one stream's data");
+    sl.sc16 = a.fmt != FMT_UC8;
+    if (sl.sc16 && !sl.d_slab) {
+        const size_t stride = ((size_t)2 + B200_TRAIL + (size_t)c->cfg.max_buffers_per_run * c->cfg.buf_samples + 32 + 127) & ~(size_t)127;
+        if (dev_alloc(&sl.d_slab, stride * S) != cudaSuccess) { sl.d_slab = nullptr; return fail(c, B200_E_NOMEM, "sc16 magnitude slab (%zu bytes)", stride * S * 2); }
+        sl.slab_stride = stride;
+    }
     sl.nseg = sl.ntile = sl.nbuf = 0; sl.is_device = true; sl.dargs = a;
     for (uint32_t s = 0; s < S; s++) {
         sl.h_stream_seg_begin[s] = sl.nseg;
         sl.stream_buf_begin[s] = sl.nbuf;
-        add_segment(c, sl, s, a.d_iq + (size_t)s * a.stride - (size_t)B200_TRAIL * 2, a.n_buffers * a.buf_len, a.buf_len, a.n_buffers,
-                    a.continues ? 0 : SEG_HALO_ZERO, a.first_ts);
+        const uint8_t *base = sl.sc16 ? reinterpret_cast<const uint8_t *>(sl.d_slab + s * sl.slab_stride + 2) : a.d_iq + (size_t)s * a.stride - (size_t)B200_TRAIL * 2;
+        add_segment(c, sl, s, base, a.n_buffers * a.buf_len, a.buf_len, a.n_buffers,
+                    (a.continues ? 0 : SEG_HALO_ZERO) | (sl.sc16 ? SEG_MAG : 0), a.first_ts);
     }
     sl.h_stream_seg_begin[S] = sl.nseg;
     sl.stream_buf_begin[S] = sl.nbuf;
-    if (c->cfg.flags & B200_CFG_MODE_AC) memset(sl.h_ac_levels, 0, (size_t)sl.nbuf * sizeof(AcLevel));      // uc8 input: the exact sums
+    if (c->cfg.flags & B200_CFG_MODE_AC) {
+        memset(sl.h_ac_levels, 0, (size_t)sl.nbuf * sizeof(AcLevel));      // uc8 input: the exact sums
+        if (sl.sc16) for (uint32_t b = 0; b < sl.nbuf; b++) {               // sc16: the converter's float sums, BufAcc::fsum of the buffer
+            sl.h_ac_levels[b].mode = AC_LEVEL_FSUM; sl.h_ac_levels[b].idx = b * (uint32_t)(sizeof(BufAcc) / sizeof(float2));
+        }
+    }
+    if (sl.sc16) {
+        Sc16Params &p = sl.conv;
+        p = Sc16Params();
+        p.iq = reinterpret_cast<const uint32_t *>(a.d_iq); p.iq_stride = a.stride / 4;
+        p.mag = sl.d_slab + 2; p.mag_stride = sl.slab_stride;
+        p.n_streams = S; p.n_buffers = a.n_buffers; p.buf_len = a.buf_len; p.halo = a.continues ? 1u : 0u;
+        p.scale = a.fmt == FMT_SC16Q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
+    }
     // the tile -> segment table only depends on the layout; skip its upload when nothing changed
-    const uint64_t key = ((uint64_t)a.n_buffers << 40) ^ ((uint64_t)a.buf_len << 8) ^ (((uintptr_t)a.d_iq >> 4) & 15) ^ (a.stride << 20);
+    const uint64_t key = ((uint64_t)a.n_buffers << 40) ^ ((uint64_t)a.buf_len << 8) ^ (((uintptr_t)a.d_iq >> 4) & 15) ^ (a.stride << 20) ^ ((uint64_t)sl.sc16 << 63);
     sl.upload_tiles = !(sl.cached_tiles == sl.ntile && sl.cached_layout_key == key);
     sl.cached_tiles = sl.ntile; sl.cached_layout_key = key;
     return B200_OK;
 }
 
-API int b200_demod_run_device_uc8(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
-                                  int continues, int64_t first_ts) {
+static int run_device(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                      int continues, int64_t first_ts, int fmt) {
     if (!c || !d_iq) return B200_E_INVAL;
     if (any_in_flight(c)) return fail(c, B200_E_STATE, "asynchronous steps are in flight: call b200_demod_wait first");
     CU(c, cudaSetDevice(c->device));
     Slot &sl = c->slot[0];
     c->cur = 0;
-    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts};
+    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts, fmt};
     int rc = build_device_run(c, sl, a);
     if (rc != B200_OK) return rc;
     return execute_blocking(c, sl);
+}
+
+API int b200_demod_run_device_uc8(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                                  int continues, int64_t first_ts) {
+    return run_device(c, d_iq, stride, n_buffers, buf_len, continues, first_ts, FMT_UC8);
+}
+
+API int b200_demod_run_device_sc16(b200_demod_ctx *c, const int16_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                                   int continues, int64_t first_ts, int q11) {
+    return run_device(c, reinterpret_cast<const uint8_t *>(d_iq), stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
 }
 
 // ---- asynchronous steps: at most NSLOT in flight ------------------------------------------------------------------------
@@ -891,8 +950,8 @@ static int launch_async(b200_demod_ctx *c, Slot &sl) {
     return B200_OK;
 }
 
-API int b200_demod_run_device_uc8_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
-                                        int continues, int64_t first_ts) {
+static int run_device_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                            int continues, int64_t first_ts, int fmt) {
     if (!c || !d_iq) return B200_E_INVAL;
     CU(c, cudaSetDevice(c->device));
     Slot &sl = c->slot[c->next_async];
@@ -901,57 +960,84 @@ API int b200_demod_run_device_uc8_async(b200_demod_ctx *c, const uint8_t *d_iq, 
         cudaError_t e = alloc_slot(c, sl, c->slot[0].rec_cap);
         if (e != cudaSuccess) return fail(c, B200_E_NOMEM, "pipeline slot %d: %s", c->next_async, cudaGetErrorString(e));
     }
-    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts};
+    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts, fmt};
     int rc = build_device_run(c, sl, a);
     if (rc != B200_OK) return rc;
     return launch_async(c, sl);
 }
 
-// ---- asynchronous host-buffer steps: the device-resident pipeline fed from two library-owned input buffers ----------
-#define PIPE_LEAD 1024        // bytes in front of each receiver's samples: the 326-sample halo sits right before them
+API int b200_demod_run_device_uc8_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                                        int continues, int64_t first_ts) {
+    return run_device_async(c, d_iq, stride, n_buffers, buf_len, continues, first_ts, FMT_UC8);
+}
 
-API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
-                                      int continues, int64_t first_ts) {
+API int b200_demod_run_device_sc16_async(b200_demod_ctx *c, const int16_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                                         int continues, int64_t first_ts, int q11) {
+    return run_device_async(c, reinterpret_cast<const uint8_t *>(d_iq), stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
+}
+
+// ---- asynchronous host-buffer steps: the device-resident pipeline fed from library-owned input buffers ----------------
+#define PIPE_LEAD 1024        // bytes in front of each receiver's samples: the 326-sample halo sits right before them
+#define PIPE_LEAD16 2048      // ... for int16 I,Q samples (326 * 4 bytes)
+
+static int run_host_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
+                          int continues, int64_t first_ts, int fmt) {
     if (!c || !h_iq) return B200_E_INVAL;
     CU(c, cudaSetDevice(c->device));
-    const uint32_t S = c->cfg.n_streams, K = c->cfg.max_buffers_per_run, BUF = c->cfg.buf_samples;
+    const uint32_t S = c->cfg.n_streams, K = c->cfg.max_buffers_per_run, BUF = c->cfg.buf_samples, bps = fmt_bytes(fmt);
     if (n_buffers == 0 || n_buffers > K || buf_len == 0 || buf_len > BUF || (buf_len & 7)) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration (buf_len must be a multiple of 8)");
-    const size_t row = (size_t)n_buffers * buf_len * 2;
+    const size_t row = (size_t)n_buffers * buf_len * bps;
     if (host_stride < row && S > 1) return fail(c, B200_E_INVAL, "host_stride_bytes smaller than one stream's data");
     for (uint32_t s = 0; s < S; s++) if (!c->pending[s].empty()) return fail(c, B200_E_STATE, "buffers submitted for b200_demod_run are pending: run them first");
     const int pi = c->next_async;
     Slot &sl = c->slot[pi];
     if (sl.in_flight) return fail(c, B200_E_STATE, "%d steps are already in flight: call b200_demod_wait", NSLOT);
-    if (continues && !c->pipe_prev_valid) return fail(c, B200_E_STATE, "continues != 0 but there is no previous run_host_uc8_async step with >= 326 samples per receiver");
+    if (continues && !(c->pipe_prev_valid && c->pipe_prev_bytes == bps))
+        return fail(c, B200_E_STATE, "continues != 0 but there is no previous %s step with >= 326 samples per receiver",
+                    fmt == FMT_UC8 ? "run_host_uc8_async" : "run_host_sc16_async");
     if (!sl.allocated) {
         cudaError_t e = alloc_slot(c, sl, c->slot[0].rec_cap);
         if (e != cudaSuccess) return fail(c, B200_E_NOMEM, "pipeline slot %d: %s", pi, cudaGetErrorString(e));
     }
-    if (!c->d_pipe[0]) {
-        c->pipe_stride = (PIPE_LEAD + (size_t)K * BUF * 2 + 64 + 255) & ~(size_t)255;
+    const size_t lead = fmt == FMT_UC8 ? PIPE_LEAD : PIPE_LEAD16;
+    uint8_t **pipe = fmt == FMT_UC8 ? c->d_pipe : c->d_pipe16;
+    size_t &pipe_stride = fmt == FMT_UC8 ? c->pipe_stride : c->pipe16_stride;
+    if (!pipe[0]) {
+        pipe_stride = (lead + (size_t)K * BUF * bps + 64 + 255) & ~(size_t)255;
         for (int i = 0; i < NSLOT; i++) {
-            if (cudaMalloc((void **)&c->d_pipe[i], c->pipe_stride * S + 256) != cudaSuccess) {
-                for (int j = 0; j < i; j++) { cudaFree(c->d_pipe[j]); c->d_pipe[j] = nullptr; }
-                return fail(c, B200_E_NOMEM, "pipelined input buffers (%d x %zu bytes)", NSLOT, c->pipe_stride * S);
+            if (cudaMalloc((void **)&pipe[i], pipe_stride * S + 256) != cudaSuccess) {
+                for (int j = 0; j < i; j++) { cudaFree(pipe[j]); pipe[j] = nullptr; }
+                pipe[i] = nullptr;
+                return fail(c, B200_E_NOMEM, "pipelined input buffers (%d x %zu bytes)", NSLOT, pipe_stride * S);
             }
-            CU(c, cudaEventCreateWithFlags(&c->ev_in[i], cudaEventDisableTiming));
+            if (!c->ev_in[i]) CU(c, cudaEventCreateWithFlags(&c->ev_in[i], cudaEventDisableTiming));
         }
     }
-    // The slot's previous step (NSLOT steps ago) has been collected, so nothing reads d_pipe[pi] any more; the copies of
+    // The slot's previous step (NSLOT steps ago) has been collected, so nothing reads pipe[pi] any more; the copies of
     // consecutive steps are ordered on in_stream, which also orders the halo copy after the previous step's samples.
-    uint8_t *dst = c->d_pipe[pi] + PIPE_LEAD;
-    CU(c, cudaMemcpy2DAsync(dst, c->pipe_stride, h_iq, host_stride, row, S, cudaMemcpyHostToDevice, c->in_stream));
+    uint8_t *dst = pipe[pi] + lead;
+    const size_t halo = (size_t)B200_TRAIL * bps;
+    CU(c, cudaMemcpy2DAsync(dst, pipe_stride, h_iq, host_stride, row, S, cudaMemcpyHostToDevice, c->in_stream));
     if (continues)      // the mag_buf overlap copy (sdr_ifile.c:209-213): the previous step's last 326 samples in front of this step's
-        CU(c, cudaMemcpy2DAsync(dst - (size_t)B200_TRAIL * 2, c->pipe_stride,
-                                c->d_pipe[c->pipe_prev] + PIPE_LEAD + c->pipe_prev_row - (size_t)B200_TRAIL * 2, c->pipe_stride,
-                                (size_t)B200_TRAIL * 2, S, cudaMemcpyDeviceToDevice, c->in_stream));
+        CU(c, cudaMemcpy2DAsync(dst - halo, pipe_stride, pipe[c->pipe_prev] + lead + c->pipe_prev_row - halo, pipe_stride,
+                                halo, S, cudaMemcpyDeviceToDevice, c->in_stream));
     CU(c, cudaEventRecord(c->ev_in[pi], c->in_stream));
     CU(c, cudaStreamWaitEvent(c->stream, c->ev_in[pi], 0));
-    c->pipe_prev = pi; c->pipe_prev_row = row; c->pipe_prev_valid = row >= (size_t)B200_TRAIL * 2;
-    const DeviceArgs a = {dst, c->pipe_stride, n_buffers, buf_len, continues ? 1 : 0, first_ts};
+    c->pipe_prev = pi; c->pipe_prev_row = row; c->pipe_prev_valid = row >= halo; c->pipe_prev_bytes = bps;
+    const DeviceArgs a = {dst, pipe_stride, n_buffers, buf_len, continues ? 1 : 0, first_ts, fmt};
     int rc = build_device_run(c, sl, a);
     if (rc != B200_OK) return rc;
     return launch_async(c, sl);
+}
+
+API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
+                                      int continues, int64_t first_ts) {
+    return run_host_async(c, h_iq, host_stride, n_buffers, buf_len, continues, first_ts, FMT_UC8);
+}
+
+API int b200_demod_run_host_sc16_async(b200_demod_ctx *c, const int16_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
+                                       int continues, int64_t first_ts, int q11) {
+    return run_host_async(c, reinterpret_cast<const uint8_t *>(h_iq), host_stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
 }
 
 // Pipelined steps keep three kernels' worth of work in flight: the scan of step n+1 (one persistent CTA per SM, the whole SM each)
@@ -965,7 +1051,8 @@ API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, ui
 // completed steps, the longest dropped), measures the winner once more and keeps it - the whole chip unless a partition wins by
 // 1.5 % and again by 1 %.  A run of a different size (tiles +- 1/8) starts over, up to four times per session.
 static void tune_partition(b200_demod_ctx *c, Slot &sl) {
-    if (c->part_fixed || c->part_off || (c->cfg.flags & B200_CFG_MODE_AC) || !sl.ntile || c->n_sm < 16) return;
+    // (sc16 steps carry a converter in front of the scan: they are not measured, as Mode A/C contexts are not)
+    if (c->part_fixed || c->part_off || (c->cfg.flags & B200_CFG_MODE_AC) || sl.sc16 || !sl.ntile || c->n_sm < 16) return;
     PartCal &k = c->cal;
     const auto now = std::chrono::steady_clock::now();
     if (!k.grids[0]) { k.grids[0] = c->n_sm; k.grids[1] = (c->n_sm * 85 + 50) / 100; k.grids[2] = (c->n_sm * 82 + 50) / 100; k.grids[3] = c->n_sm; k.skip = 8; }

@@ -54,6 +54,9 @@ def lib():
         L.b200_demod_run_device_uc8.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64]
         L.b200_demod_run_device_uc8_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64]
         L.b200_demod_run_host_uc8_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64]
+        L.b200_demod_run_device_sc16.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
+        L.b200_demod_run_device_sc16_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
+        L.b200_demod_run_host_sc16_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
         L.b200_demod_wait.argtypes = [vp]
         L.b200_demod_frame_count.argtypes = [vp, u32, C.POINTER(u32)]
         L.b200_demod_fetch.argtypes = [vp, u32, vp, u32, C.POINTER(u32)]
@@ -83,6 +86,7 @@ EXPORTED_SYMBOLS = [
     "b200_demod_uc8_lut", "b200_demod_debug_counters", "b200_demod_submit_iq_uc8_strided", "b200_demod_set_stream",
     "b200_demod_run_device_uc8_async", "b200_demod_wait", "b200_demod_fetch_modeac", "b200_demod_run_host_uc8_async",
     "b200_demod_submit_mag_u16_levels", "b200_demod_set_preamble_threshold",
+    "b200_demod_run_device_sc16", "b200_demod_run_device_sc16_async", "b200_demod_run_host_sc16_async",
 ]
 
 
@@ -194,6 +198,22 @@ class Demodulator:
         sdr_ifile.c:194-259): the host slab is copied on a stream of its own while the previous step's kernels run."""
         self._check(self.L.b200_demod_run_host_uc8_async(self.h, h_ptr, host_stride_bytes, n_buffers, buf_len,
                                                          1 if continues else 0, first_sample_timestamp))
+
+    def run_device_sc16(self, d_ptr: int, stream_stride_bytes: int, n_buffers: int, buf_len: int, continues: bool,
+                        first_sample_timestamp: int, q11: bool = False):
+        """run_device for int16 I,Q input (convert_sc16_nodc, or convert_sc16q11_nodc with q11): 4 bytes per sample."""
+        self._check(self.L.b200_demod_run_device_sc16(self.h, d_ptr, stream_stride_bytes, n_buffers, buf_len,
+                                                      1 if continues else 0, first_sample_timestamp, 1 if q11 else 0))
+
+    def run_device_sc16_async(self, d_ptr: int, stream_stride_bytes: int, n_buffers: int, buf_len: int, continues: bool,
+                              first_sample_timestamp: int, q11: bool = False):
+        self._check(self.L.b200_demod_run_device_sc16_async(self.h, d_ptr, stream_stride_bytes, n_buffers, buf_len,
+                                                            1 if continues else 0, first_sample_timestamp, 1 if q11 else 0))
+
+    def run_host_sc16_async(self, h_ptr: int, host_stride_bytes: int, n_buffers: int, buf_len: int, continues: bool,
+                            first_sample_timestamp: int, q11: bool = False):
+        self._check(self.L.b200_demod_run_host_sc16_async(self.h, h_ptr, host_stride_bytes, n_buffers, buf_len,
+                                                          1 if continues else 0, first_sample_timestamp, 1 if q11 else 0))
 
     def wait(self):
         self._check(self.L.b200_demod_wait(self.h))
