@@ -262,6 +262,52 @@ int b200_demod_run_host_sc16_async(b200_demod_ctx *ctx, const int16_t *h_iq, uin
                                    uint32_t n_buffers, uint32_t buf_len, int continues,
                                    int64_t first_sample_timestamp, int q11);
 
+/* independent live receivers in one step ------------------------------------------------------
+ * The calls above give every receiver of a step the same buffer count, timestamp, halo rule and threshold.  Live SDRs are not in
+ * lockstep: they start at different times, their sample clocks drift, and each drops blocks on its own when readsb's FIFO is full
+ * (sdr_rtlsdr.c:345-359; the buffer after a drop starts with a zero halo, sdr_rtlsdr.c:381-385, and while samples were dropped
+ * recently the receiver's preamble threshold is at least 75, demod_2400.c:334-338).  The _rx calls take one descriptor per receiver
+ * of the context (rx[0 .. n_streams-1]). */
+typedef struct b200_rx_step {
+    int64_t  first_sample_timestamp; /* this receiver's 12 MHz clock at its first new sample */
+    uint32_t n_buffers;              /* buffers this receiver delivers in this step, 0 .. max_buffers_per_run; 0 = not in this step */
+    uint32_t flags;                  /* B200_RX_CONTINUES: these samples follow this receiver's previous ones without a gap */
+    int32_t  preamble_threshold;     /* 0: the context's (b200_demod_set_preamble_threshold); else this receiver's, > 0 */
+    uint32_t reserved_;              /* must be 0 */
+} b200_rx_step;                      /* 24 bytes */
+#define B200_RX_CONTINUES 0x1u
+enum { B200_FORMAT_UC8 = 0, B200_FORMAT_SC16 = 1, B200_FORMAT_SC16Q11 = 2 };
+
+/* format: B200_FORMAT_UC8 (uc8 I,Q, 2 bytes per sample), _SC16 or _SC16Q11 (int16 I,Q, 4 bytes per sample, converted as by
+ * b200_demod_run_device_sc16 with q11 = 0 / 1).  Receiver s's rx[s].n_buffers * buf_len samples start at d_iq + s * stream_stride_bytes
+ * (h_iq + s * host_stride_bytes) and are processed as rx[s].n_buffers consecutive buffers of buf_len samples with timestamps
+ * rx[s].first_sample_timestamp + b * buf_len * 5; the stride must hold the largest count of the step.  d_iq and stream_stride_bytes
+ * 16-byte aligned, buf_len a multiple of 8, at most buf_samples, as for the calls above.
+ *   B200_RX_CONTINUES, device path: the 326 samples in front of the receiver's first sample are valid halo (else: zero halo).
+ *   B200_RX_CONTINUES, host path: the receiver's last run_host_* step of the same sample width (uc8 or sc16) gives the halo, also if the
+ *     receiver was absent from the steps in between; that step must have left it >= 326 samples, else B200_E_STATE.  The library keeps
+ *     every receiver's last 326 raw samples in a store of its own (allocated with the pipelined input buffers).  The host slab is copied
+ *     in one strided copy of the largest count's bytes per receiver: every row must be readable that far.
+ *   n_buffers == 0: the receiver is absent: no buffer results, no frames; its filter, flip clock, buffer sequence and (host path)
+ *     stored halo stay as they are.  A step may leave every receiver absent.
+ *   preamble_threshold: what demod_2400.c:334-338 uses for this receiver's buffers of this step (e.g. max(75, threshold) while its
+ *     samples_dropped is non-zero); 0 = the context's.
+ * Refused with B200_E_INVAL before anything is enqueued or changed (no halo stored, no pipeline slot taken): a bad format, n_buffers
+ * above max_buffers_per_run, a negative threshold, non-zero reserved_ or unknown flag bits, a stride too small for the largest count,
+ * and the alignment / buf_len rules.  Results, waits and pipelining as for the calls above; the uniform calls are these calls with
+ * one descriptor repeated. */
+int b200_demod_run_device_rx(b200_demod_ctx *ctx, int format, const void *d_iq, uint64_t stream_stride_bytes, uint32_t buf_len,
+                             const b200_rx_step *rx);
+int b200_demod_run_device_rx_async(b200_demod_ctx *ctx, int format, const void *d_iq, uint64_t stream_stride_bytes, uint32_t buf_len,
+                                   const b200_rx_step *rx);
+int b200_demod_run_host_rx_async(b200_demod_ctx *ctx, int format, const void *h_iq, uint64_t host_stride_bytes, uint32_t buf_len,
+                                 const b200_rx_step *rx);
+/* The host-buffer path's form of a dropped block (sdr_rtlsdr.c:381-385, oracle_stream_restart): the receiver's next buffer given to
+ * submit_iq_uc8 / submit_iq_uc8_strided / submit_iq_sc16 starts with a zero halo instead of the previous buffer's tail.  Buffers of
+ * the same run already pending keep theirs; the restart falls between them and the next one.  No effect on magnitude hand-offs,
+ * which bring their halo with them. */
+int b200_demod_restart_stream(b200_demod_ctx *ctx, uint32_t stream);
+
 /* results of the last run ---------------------------------------------------------------------- */
 int b200_demod_frame_count(b200_demod_ctx *ctx, uint32_t stream, uint32_t *n);
 int b200_demod_fetch(b200_demod_ctx *ctx, uint32_t stream, b200_frame *out, uint32_t cap, uint32_t *n);

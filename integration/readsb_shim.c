@@ -103,8 +103,10 @@ void __wrap_demodulate2400(struct mag_buf *mag) {
     unsigned iq_n = 0;
     int rc_submit;
     if (b200_shim_iq_lookup && b200_shim_iq_lookup(mag->data + Modes.trailing_samples, &iq, &iq_n) && iq_n == mag->length) {
-        /* converter hook active: the frontend's raw uc8 IQ goes up, convert_uc8_nodc (convert.c:64-108) runs on the GPU */
-        rc_submit = b200_demod_submit_iq_uc8(g_ctx, 0, iq, mag->length, mag->sampleTimestamp);
+        /* converter hook active: the frontend's raw uc8 IQ goes up, convert_uc8_nodc (convert.c:64-108) runs on the GPU.  The library
+         * keeps the halo on this branch: after dropped samples it must start from zeros, as sdr_rtlsdr.c:381-385 does */
+        rc_submit = mag->dropped ? b200_demod_restart_stream(g_ctx, 0) : B200_OK;
+        if (rc_submit == B200_OK) rc_submit = b200_demod_submit_iq_uc8(g_ctx, 0, iq, mag->length, mag->sampleTimestamp);
     } else {
         iq = NULL;
         pin_once(mag);

@@ -67,6 +67,13 @@ BUFRES_DTYPE = np.dtype([("sample_timestamp", "<i8"), ("sum_level", "<u8"), ("su
                          ("pad_", "<u4")])
 assert FRAME_DTYPE.itemsize == 64 and BUFRES_DTYPE.itemsize == 112
 
+# b200_rx_step: one receiver's part of a step of the _rx calls (include/b200_demod.h)
+RX_STEP_DTYPE = np.dtype([("first_sample_timestamp", "<i8"), ("n_buffers", "<u4"), ("flags", "<u4"), ("preamble_threshold", "<i4"),
+                          ("reserved_", "<u4")])
+assert RX_STEP_DTYPE.itemsize == 24
+RX_CONTINUES = 0x1
+FORMAT_UC8, FORMAT_SC16, FORMAT_SC16Q11 = 0, 1, 2
+
 # fields of a frame that the reference itself defines (flags is this library's own annotation)
 FRAME_PARITY_FIELDS = ("timestamp", "sigpow_sum", "j", "crc", "addr", "score", "buffer_seq", "signal_len",
                        "phase", "msgtype", "msgbits", "correctedbits", "fix_bit", "msg")

@@ -40,7 +40,8 @@ struct Segment {
     uint32_t tile_begin;   // global index of this segment's first tile
     uint32_t n_tiles;
     uint32_t first_seq;    // buffer_seq of the segment's first buffer
-    uint32_t pad_[2];
+    int32_t  thr;          // the receiver's Modes.preambleThreshold for this segment (demod_2400.c:334-338)
+    uint32_t pad_;
 };
 
 // One position whose preamble correlation reached the threshold (demod_2400.c:344-378).
@@ -153,7 +154,6 @@ struct ScanParams {
     uint32_t need_lut;           // some segment holds uc8 IQ: the magnitude table has to be staged (a pure magnitude hand-off skips it)
     uint32_t sub_chunks;         // caller: chunks of 512 positions per warp it asks for when the run is small (0: whole tiles); the launcher
                                  // keeps it only with static_tiles: the TILE_CHUNKS / sub_chunks first warps of CTA b share tile b
-    int32_t thr;                 // Modes.preambleThreshold
     uint32_t long_set, short_set; // valid DF bitsets (demod_2400.c:98-128)
     int32_t nfix, fixdf;
     // per-warp private areas in global memory
@@ -263,14 +263,17 @@ struct AcWalkParams {
 };
 
 // ---- sc16 / sc16q11 input (convert_kernel.cu) ----------------------------------------------------
-// Buffer g = s * n_buffers + b of a step: receiver s, its buffer b.  Samples are interleaved int16 I,Q (one 32-bit word each).
+// Buffer g of a step belongs to the segment whose buffers [first_buf, first_buf + n_bufs) hold it: receiver seg.stream, its buffer
+// g - seg.first_buf.  Samples are interleaved int16 I,Q (one 32-bit word each).
 struct Sc16Params {
-    const uint32_t *iq;               // receiver s's first new sample at iq + s * iq_stride; with `halo` its 326 raw halo samples precede it
+    const uint32_t *iq;               // receiver s's first new sample at iq + s * iq_stride; unless its segment has SEG_HALO_ZERO, its 326 raw
+                                      // halo samples precede it and are converted too
     uint16_t *mag;                    // receiver s's data index 0 (first halo magnitude) at mag + s * mag_stride
     float2 *sums;                     // buffer g's float sums (sum_level, sum_power) at sums[g * sums_stride]
+    const Segment *segs;              // the step's segments (one per receiver present), ascending first_buf; not read when n_segs == 1
+    Segment seg0;                     // ... the only one when n_segs == 1 (its descriptors may not be on the device)
     uint64_t iq_stride, mag_stride;   // in samples
-    uint32_t sums_stride, n_streams, n_buffers, buf_len;
-    uint32_t halo;                    // also convert the halo (the step continues its receivers)
+    uint32_t sums_stride, n_segs, n_bufs, buf_len;
     float scale;                      // 1 / 32768 (sc16) or 1 / 2048 (sc16q11)
 };
 

@@ -41,22 +41,32 @@ __device__ __forceinline__ uint16_t sc16_mag_u16(float mag) {
     return (uint16_t)(scaled + 0.5f);
 }
 
-__global__ void __launch_bounds__(SC16_WORKERS + 32, 1) sc16_convert_kernel(const Sc16Params P) {
-    extern __shared__ __align__(16) float sc16_stage[];       // [2][2 * SC16_GROUP][SC16_ROW]
-    const uint32_t tid = threadIdx.x;
-    const uint32_t nbuf = P.n_streams * P.n_buffers, g0 = blockIdx.x * SC16_GROUP;
-    const uint32_t n_here = min((uint32_t)SC16_GROUP, nbuf - g0);
+// The segment that holds buffer g (the last one whose first_buf <= g): receivers present in the step hold one segment each, in order.
+__device__ __forceinline__ const Segment &sc16_seg(const Sc16Params &P, uint32_t i) { return P.n_segs == 1 ? P.seg0 : P.segs[i]; }
 
-    // halos of the receivers whose first buffer is in this CTA: converted, not summed
-    if (P.halo) {
-        for (uint32_t s = (g0 + P.n_buffers - 1) / P.n_buffers; s * P.n_buffers < g0 + n_here; s++) {
-            const uint32_t *in = P.iq + s * P.iq_stride - B200_TRAIL;
-            uint16_t *out = P.mag + s * P.mag_stride;
-            for (uint32_t i = tid; i < B200_TRAIL; i += blockDim.x) {
-                float mag, magsq;
-                sc16_sample(in[i], P.scale, mag, magsq);
-                out[i] = sc16_mag_u16(mag);
-            }
+__global__ void __launch_bounds__(SC16_WORKERS + 32, 1) sc16_convert_kernel(const __grid_constant__ Sc16Params P) {
+    extern __shared__ __align__(16) float sc16_stage[];       // [2][2 * SC16_GROUP][SC16_ROW]
+    __shared__ uint32_t grp_seg[SC16_GROUP];                  // segment of buffer g0 + j
+    const uint32_t tid = threadIdx.x;
+    const uint32_t nbuf = P.n_bufs, g0 = blockIdx.x * SC16_GROUP;
+    const uint32_t n_here = min((uint32_t)SC16_GROUP, nbuf - g0);
+    if (tid < n_here) {
+        uint32_t lo = 0, hi = P.n_segs;                       // invariant: first_buf(lo) <= g < first_buf(hi)
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) / 2; if (sc16_seg(P, mid).first_buf <= g0 + tid) lo = mid; else hi = mid; }
+        grp_seg[tid] = lo;
+    }
+    __syncthreads();
+
+    // halos of the continued receivers whose first buffer is in this CTA: converted, not summed
+    for (uint32_t j = 0; j < n_here; j++) {
+        const Segment &sg = sc16_seg(P, grp_seg[j]);
+        if (sg.first_buf != g0 + j || (sg.flags & SEG_HALO_ZERO)) continue;
+        const uint32_t *in = P.iq + sg.stream * P.iq_stride - B200_TRAIL;
+        uint16_t *out = P.mag + sg.stream * P.mag_stride;
+        for (uint32_t i = tid; i < B200_TRAIL; i += blockDim.x) {
+            float mag, magsq;
+            sc16_sample(in[i], P.scale, mag, magsq);
+            out[i] = sc16_mag_u16(mag);
         }
     }
 
@@ -67,7 +77,9 @@ __global__ void __launch_bounds__(SC16_WORKERS + 32, 1) sc16_convert_kernel(cons
         uint16_t *dst[SC16_GROUP];
 #pragma unroll
         for (int j = 0; j < SC16_GROUP; j++) {
-            const uint32_t g = g0 + min((uint32_t)j, n_here - 1), s = g / P.n_buffers, b = g % P.n_buffers;
+            const uint32_t jj = min((uint32_t)j, n_here - 1);
+            const Segment &sg = sc16_seg(P, grp_seg[jj]);
+            const uint32_t s = sg.stream, b = g0 + jj - sg.first_buf;
             src[j] = P.iq + s * P.iq_stride + (size_t)b * P.buf_len;
             dst[j] = P.mag + s * P.mag_stride + B200_TRAIL + (size_t)b * P.buf_len;
         }
@@ -126,7 +138,7 @@ extern "C" int b200_prepare_convert(void) {      // per device, from b200_demod_
 }
 
 extern "C" int b200_launch_sc16_convert(const Sc16Params *p, void *stream) {
-    const uint32_t nbuf = p->n_streams * p->n_buffers;
+    const uint32_t nbuf = p->n_bufs;
     if (!nbuf || !p->buf_len) return 0;
     sc16_convert_kernel<<<(nbuf + SC16_GROUP - 1) / SC16_GROUP, SC16_WORKERS + 32, SC16_SMEM, (cudaStream_t)stream>>>(*p);
     return (int)cudaGetLastError();

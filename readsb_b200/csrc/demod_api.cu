@@ -33,6 +33,7 @@ struct Pending {
     int64_t ts;
     size_t off;          // byte offset of data index 0 (mag) or of the first new sample (iq) in the stream's arena region
     int fsum = -1;       // sc16 input: index of the buffer's float sums in d_fsum
+    bool restart = false;                // iq input: b200_demod_restart_stream came before this buffer (zero halo)
     bool has_levels = false;             // magnitude hand-off with the mag_buf's own mean_level / mean_power (Mode A/C noise floor)
     double mean_level = 0, mean_power = 0;
 };
@@ -40,10 +41,6 @@ struct Pending {
 // sample format of a device-resident or pipelined step
 enum IqFormat { FMT_UC8 = 0, FMT_SC16 = 1, FMT_SC16Q11 = 2 };
 static inline uint32_t fmt_bytes(int fmt) { return fmt == FMT_UC8 ? 2u : 4u; }     // bytes per raw sample
-
-struct DeviceArgs {      // what a device-resident step was asked to do (kept for a repeat after a pool regrowth)
-    const uint8_t *d_iq; uint64_t stride; uint32_t n_buffers, buf_len; int continues; int64_t first_ts; int fmt;
-};
 
 struct Slot {
     bool allocated = false, in_flight = false, completed = false;
@@ -54,13 +51,15 @@ struct Slot {
     //   result block      [RunCtl | buf_acc (nbuf) | frame_span (2S) | buf_out (nbuf) | packed frames ...]
     uint8_t *d_desc = nullptr, *h_desc = nullptr, *d_res = nullptr, *h_res = nullptr;
     uint8_t *d_res_host = nullptr;    // h_res as the device sees it (mapped pinned memory): the one-receiver kernel publishes its results there
-    bool res_clean = false;           // RunCtl + BufAcc[] in d_res are zero (the one-receiver kernel cleans up after itself)
+    bool res_clean = false;           // RunCtl + BufAcc[0 .. clean_bufs) in d_res are zero (the one-receiver kernel cleans up after itself)
+    uint32_t clean_bufs = 0;
     size_t desc_cap = 0, res_cap = 0, res_head = 0;     // res_head: bytes in front of the packed frames in this run's result block
     Segment *d_segs = nullptr, *h_segs = nullptr;       // h_segs / h_tile_seg / h_stream_seg_begin: where the host BUILDS the run (copied into h_desc)
     uint32_t *d_tile_seg = nullptr, *h_tile_seg = nullptr;
     uint32_t *d_stream_seg_begin = nullptr, *h_stream_seg_begin = nullptr;
     uint32_t cached_tiles = 0;        // tile_seg on the device is valid for this many tiles (device-resident path)
     uint64_t cached_layout_key = 0;
+    std::vector<uint32_t> cached_counts;      // ... and these per-receiver buffer counts
     RunCtl *d_ctl = nullptr, *h_ctl = nullptr;
     PosEntry *d_pos_pool = nullptr;
     Rec *d_rec_pool = nullptr;
@@ -80,8 +79,7 @@ struct Slot {
     // the run this slot holds
     uint32_t nseg = 0, ntile = 0, nbuf = 0, run_frames = 0;
     size_t desc_bytes = 0;            // bytes of the descriptor block this run uploads
-    bool upload_tiles = true, is_device = false;
-    DeviceArgs dargs = {};
+    bool upload_tiles = true;
     std::vector<uint32_t> stream_buf_begin;   // [n_streams+1] into h_buf_out
     cudaEvent_t ev[8] = {};                   // 0 scan begin, 1 scan end, 2 resolve end, 3 finalize end, 4 results on host,
                                               // 5 result copies done, 6 Mode A/C scan + walk done, 7 descriptors uploaded
@@ -142,6 +140,7 @@ struct b200_demod_ctx {
     std::vector<std::vector<Pending>> pending;
     std::vector<uint8_t> kind;        // per stream this run: 0 none, 1 uc8 iq, 2 mag hand-off, 3 sc16 iq (magnitudes made by the library)
     std::vector<uint8_t> halo_valid;  // iq streams: saved 326-sample tail is valid
+    std::vector<uint8_t> restart_next;  // iq streams: the next submitted buffer starts with a zero halo (b200_demod_restart_stream)
     std::vector<size_t> cursor;       // append offset in the stream's arena region
 
     uint32_t seg_cap = 0, tile_cap = 0, buf_cap = 0, frame_cap = 0, ac_cap = 0;
@@ -171,9 +170,12 @@ struct b200_demod_ctx {
     uint8_t *d_pipe16[NSLOT] = {};    // ... the same for run_host_sc16_async (int16 samples), allocated on its first step
     size_t pipe16_stride = 0;
     cudaEvent_t ev_in[NSLOT] = {};
-    bool pipe_prev_valid = false;     // the buffer of the previous step holds >= 326 samples per receiver
-    int pipe_prev = 0; size_t pipe_prev_row = 0;
-    uint32_t pipe_prev_bytes = 0;     // bytes per sample of the previous step (2 uc8, 4 sc16): a halo only continues the same input width
+    // ... and each receiver's halo between its host-buffer steps: its last 326 raw samples (halo_store_kernel)
+    uint16_t *d_halo_store = nullptr;                // [S][326 * 4 bytes]
+    uint32_t *d_halo_op = nullptr, *h_halo_op = nullptr;     // [NSLOT][S] what halo_store_kernel does for each receiver in that slot's step
+    std::vector<uint8_t> halo_bytes;  // per receiver: bytes per sample of its stored halo (2 uc8, 4 sc16), 0 = none; a halo only
+                                      // continues a step of the same input width
+    std::vector<b200_rx_step> rx_uniform;     // the uniform calls' descriptor array
 };
 
 static int fail(b200_demod_ctx *c, int code, const char *fmt, ...) {
@@ -200,6 +202,19 @@ __global__ void carry_halo_kernel(uint8_t *arena, size_t stride, const uint32_t 
     const uint16_t *from = reinterpret_cast<const uint16_t *>(region + src[s]);
     uint16_t *to = reinterpret_cast<uint16_t *>(region);
     for (uint32_t i = threadIdx.x; i < B200_TRAIL; i += blockDim.x) to[i] = from[i];
+}
+
+// Host-buffer steps (run_host_*_async): the mag_buf overlap copy (sdr_ifile.c:209-213) of every receiver through a halo store of its
+// own, so that a receiver continues its own last step whatever steps it was absent from.  One block per receiver; its first new
+// sample at slab + s * stride, op[s] = new samples << 1 | continues, 0 = absent.  A continued receiver first gets its stored
+// 326 raw samples in front of its new ones; a receiver with >= 326 new samples then stores its last 326 for its next step.
+__global__ void halo_store_kernel(uint8_t *slab, size_t stride, uint16_t *store, const uint32_t *op, uint32_t bps) {
+    const uint32_t s = blockIdx.x, o = op[s], n = o >> 1, n16 = B200_TRAIL * bps / 2;
+    uint16_t *halo = reinterpret_cast<uint16_t *>(slab + (size_t)s * stride) - n16;      // the halo, then the new samples
+    uint16_t *st = store + (size_t)s * (B200_TRAIL * 2);
+    if (o & 1u) for (uint32_t i = threadIdx.x; i < n16; i += blockDim.x) halo[i] = st[i];
+    __syncthreads();
+    if (n >= B200_TRAIL) for (uint32_t i = threadIdx.x; i < n16; i += blockDim.x) st[i] = halo[n * bps / 2 + i];
 }
 
 API int b200_demod_abi_version(void) { return B200_DEMOD_ABI_VERSION; }
@@ -321,6 +336,7 @@ API void b200_demod_destroy(b200_demod_ctx *c) {
     cudaFree(c->d_stage_rec); cudaFree(c->d_stage_key); cudaFree(c->d_q1_over); cudaFree(c->d_tick_scratch);
     cudaFreeHost(c->h_carry_src); cudaFreeHost(c->h_zero);
     cudaFree(c->d_raw16); cudaFree(c->d_fsum); cudaFreeHost(c->h_fsum);
+    cudaFree(c->d_halo_store); cudaFree(c->d_halo_op); cudaFreeHost(c->h_halo_op);
     cudaFree(c->d_beast); cudaFree(c->d_beast_meta); cudaFreeHost(c->h_beast); cudaFreeHost(c->h_beast_meta);
     for (Slot &sl : c->slot) free_slot(sl);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -404,6 +420,7 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
     CUC(cudaMalloc((void **)&c->d_arena, c->stream_stride * S + 256));
     CUC(cudaMemsetAsync(c->d_arena, 0, c->stream_stride * S + 256, c->stream));
     c->pending.resize(S); c->kind.assign(S, 0); c->halo_valid.assign(S, 0); c->cursor.assign(S, 0);
+    c->restart_next.assign(S, 0); c->halo_bytes.assign(S, 0); c->rx_uniform.resize(S);
 
     const uint32_t tiles_per_buf = (BUF + 16 + SCAN_TILE - 1) / SCAN_TILE + 1;
     c->seg_cap = S * K;
@@ -446,7 +463,8 @@ static int submit_common(b200_demod_ctx *c, uint32_t s, const void *host, uint32
     if (!c->kind[s]) { c->kind[s] = want; c->cursor[s] = mag ? 0 : (size_t)B200_TRAIL * 2; }
     uint8_t *region = c->d_arena + (size_t)s * c->stream_stride;
     Pending p;
-    p.n = n; p.ts = ts;
+    p.n = n; p.ts = ts; p.restart = c->restart_next[s] != 0;
+    c->restart_next[s] = 0;               // (a magnitude hand-off brings its own halo: nothing to restart)
     if (levels) { p.has_levels = true; p.mean_level = levels[0]; p.mean_power = levels[1]; }
     if (mag) {
         p.off = (c->cursor[s] + 15) & ~(size_t)15;
@@ -492,8 +510,10 @@ API int b200_demod_submit_iq_uc8_strided(b200_demod_ctx *c, uint32_t first, uint
         c->kind[s] = 1;
         for (uint32_t b = 0; b < n_buffers; b++) {
             Pending p; p.n = buf_len; p.ts = ts + (int64_t)b * buf_len * 5; p.off = off0 + (size_t)b * buf_len * 2;
+            p.restart = b == 0 && c->restart_next[s];
             c->pending[s].push_back(p);
         }
+        c->restart_next[s] = 0;
         c->cursor[s] = off0 + row;
     }
     return B200_OK;
@@ -515,17 +535,26 @@ API int b200_demod_submit_iq_sc16(b200_demod_ctx *c, uint32_t s, const int16_t *
     if (!c->kind[s]) { c->kind[s] = 3; c->cursor[s] = (size_t)B200_TRAIL * 2; }
     uint8_t *region = c->d_arena + (size_t)s * c->stream_stride;
     Pending p;
-    p.n = n; p.ts = ts; p.off = c->cursor[s]; p.fsum = (int)c->n_fsum++;
+    p.n = n; p.ts = ts; p.off = c->cursor[s]; p.fsum = (int)c->n_fsum++; p.restart = c->restart_next[s] != 0;
     // one staging buffer: the copy and the converter of this submit are ordered on the stream before the next submit's copy
     if (n) CU(c, cudaMemcpyAsync(c->d_raw16, iq, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
     Sc16Params cp = {};
     cp.iq = reinterpret_cast<const uint32_t *>(c->d_raw16); cp.mag = reinterpret_cast<uint16_t *>(region + p.off) - B200_TRAIL;
-    cp.sums = c->d_fsum + p.fsum; cp.sums_stride = 1; cp.n_streams = 1; cp.n_buffers = 1; cp.buf_len = n;
+    cp.sums = c->d_fsum + p.fsum; cp.sums_stride = 1; cp.n_segs = 1; cp.n_bufs = 1; cp.buf_len = n;
+    cp.seg0.flags = SEG_HALO_ZERO;        // buffer 0 of receiver 0 (here: this buffer); its halo is already in the arena
     cp.scale = q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
     { int r = b200_launch_sc16_convert(&cp, c->stream);
       if (r) return fail(c, B200_E_CUDA, "sc16 convert launch: %s", cudaGetErrorString((cudaError_t)r)); }
     c->cursor[s] = p.off + (size_t)n * 2;
     c->pending[s].push_back(p);
+    c->restart_next[s] = 0;
+    return B200_OK;
+}
+
+API int b200_demod_restart_stream(b200_demod_ctx *c, uint32_t s) {
+    if (!c) return B200_E_INVAL;
+    if (s >= c->cfg.n_streams) return fail(c, B200_E_INVAL, "bad stream");
+    c->restart_next[s] = 1;               // read by the next submit_iq_* of this receiver (oracle_stream_restart)
     return B200_OK;
 }
 
@@ -545,12 +574,11 @@ API int b200_demod_set_preamble_threshold(b200_demod_ctx *c, int32_t thr) {
 }
 
 // ---- the pipeline ------------------------------------------------------------------------------
-static void add_segment(b200_demod_ctx *c, Slot &sl, uint32_t stream, const uint8_t *base, uint32_t npos, uint32_t buf_len, uint32_t n_bufs,
-                        uint32_t flags, int64_t first_ts) {
-    (void)c;
+static void add_segment(Slot &sl, uint32_t stream, const uint8_t *base, uint32_t npos, uint32_t buf_len, uint32_t n_bufs,
+                        uint32_t flags, int64_t first_ts, int32_t thr) {
     Segment &g = sl.h_segs[sl.nseg];
     memset(&g, 0, sizeof g);
-    g.base = base; g.first_ts = first_ts; g.npos = npos; g.buf_len = buf_len ? buf_len : 1;
+    g.base = base; g.first_ts = first_ts; g.thr = thr; g.npos = npos; g.buf_len = buf_len ? buf_len : 1;
     g.lead = (uint32_t)(((uintptr_t)base & 15) / 2); g.flags = flags; g.stream = stream;
     g.first_buf = sl.nbuf; g.n_bufs = n_bufs; g.tile_begin = sl.ntile;
     g.n_tiles = npos ? (g.lead + npos + SCAN_TILE - 1) / SCAN_TILE : 0;
@@ -580,7 +608,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     const bool timing = !((c->cfg.flags & B200_CFG_NO_TIMING) && scan == res);
     // Control block + per-buffer sums: zeroed by a copy engine.  (A memset runs on the SMs, and while the step before this one keeps
     // them busy it would hold this step's scan kernel back.)
-    if (!(publish && sl.res_clean))
+    if (!(publish && sl.res_clean && sl.nbuf <= sl.clean_bufs))
         CU(c, cudaMemcpyAsync(sl.d_res, c->h_zero, sizeof(RunCtl) + (size_t)sl.nbuf * sizeof(BufAcc), cudaMemcpyHostToDevice, pre));
     sl.res_clean = false; sl.published = publish; sl.timed = timing;
     if (pre != scan) { CU(c, cudaEventRecord(sl.ev[7], pre)); CU(c, cudaStreamWaitEvent(scan, sl.ev[7], 0)); }
@@ -588,7 +616,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
 
     ScanParams sp;
     sp.segs = sl.d_segs; sp.tile_seg = sl.d_tile_seg; sp.n_tiles = sl.ntile; sp.pos_pool = sl.d_pos_pool; sp.rec_pool = sl.d_rec_pool;
-    sp.key_pool = sl.d_key_pool; sp.tile_out = sl.d_tile_out; sp.buf_acc = sl.d_buf_acc; sp.ctl = sl.d_ctl; sp.thr = c->cfg.preamble_threshold;
+    sp.key_pool = sl.d_key_pool; sp.tile_out = sl.d_tile_out; sp.buf_acc = sl.d_buf_acc; sp.ctl = sl.d_ctl;
     sp.rec_cap = sl.rec_cap; sp.warps_per_cta = 0; sp.static_tiles = 0; sp.need_lut = 0; sp.sub_chunks = (uint32_t)c->scan_sub;
     sp.one_seg_valid = one_seg ? 1u : 0u;
     if (sl.nseg) sp.one_seg = sl.h_segs[0]; else memset(&sp.one_seg, 0, sizeof sp.one_seg);
@@ -603,7 +631,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     if (sp.nfix && sp.fixdf) for (int b = 0; b < 5; b++) sp.long_set |= 1u << (17 ^ (1 << b));
     if (timing) CU(c, cudaEventRecord(sl.ev[0], scan));
     if (sl.sc16) {          // after the zeroing of the per-buffer sums above: the converter writes BufAcc::fsum
-        sl.conv.sums = &sl.d_buf_acc->fsum; sl.conv.sums_stride = sizeof(BufAcc) / sizeof(float2);
+        sl.conv.sums = &sl.d_buf_acc->fsum; sl.conv.sums_stride = sizeof(BufAcc) / sizeof(float2); sl.conv.segs = sl.d_segs;
         int r = b200_launch_sc16_convert(&sl.conv, scan); if (r) return fail(c, B200_E_CUDA, "sc16 convert launch: %s", cudaGetErrorString((cudaError_t)r));
         sl.launches++;
     }
@@ -676,7 +704,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
 // because the step before it had to be repeated, 4 = a receiver's ICAO filter tables have to grow first.
 static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
     if (sl.timed) CU(c, cudaEventSynchronize(sl.ev[4])); else CU(c, cudaStreamSynchronize(res));
-    if (sl.published) sl.res_clean = true;               // the kernel zeroed RunCtl + BufAcc[] after publishing them
+    if (sl.published) { sl.res_clean = true; sl.clean_bufs = sl.nbuf; }     // the kernel zeroed RunCtl + BufAcc[] after publishing them
     const uint32_t ov = sl.h_ctl->overflow;
     if (ov & 1u) return 1;
     if ((ov & 2u) && sl.h_ctl->stage_need > c->stage_cap) return 2;
@@ -793,7 +821,8 @@ API int b200_demod_run(b200_demod_ctx *c) {
     const uint32_t S = c->cfg.n_streams, BUF = c->cfg.buf_samples;
     Slot &sl = c->slot[0];
     c->cur = 0;
-    sl.nseg = sl.ntile = sl.nbuf = 0; sl.is_device = false; sl.upload_tiles = true; sl.cached_tiles = 0; sl.sc16 = false;
+    sl.nseg = sl.ntile = sl.nbuf = 0; sl.upload_tiles = true; sl.cached_tiles = 0; sl.sc16 = false;
+    const int32_t thr = c->cfg.preamble_threshold;
     std::vector<std::pair<uint32_t, int>> fsum_of_buf;      // (buffer of the run, float-sum slot) for sc16 buffers
     std::vector<std::pair<uint32_t, const Pending *>> given_levels;   // (buffer of the run, hand-off that brought its own mean_level / mean_power)
     std::vector<uint8_t> halo_after(c->halo_valid);        // committed only when the run succeeded (a failed run leaves no halo behind)
@@ -807,7 +836,7 @@ API int b200_demod_run(b200_demod_ctx *c) {
         if (c->kind[s] == 2) {
             for (const Pending &p : pl) {
                 if (p.has_levels) given_levels.push_back({sl.nbuf, &p});
-                add_segment(c, sl, s, region + p.off, p.n, p.n, 1, SEG_MAG, p.ts);
+                add_segment(sl, s, region + p.off, p.n, p.n, 1, SEG_MAG, p.ts, thr);
             }
         } else {
             // consecutive full buffers with contiguous timestamps form one segment; a partial buffer ends it
@@ -816,15 +845,16 @@ API int b200_demod_run(b200_demod_ctx *c) {
             while (i < pl.size()) {
                 size_t j = i;
                 uint32_t npos = 0;
+                if (pl[i].restart) halo_ok = false;        // sdr_rtlsdr.c:381-385: a buffer after dropped samples starts with a zero halo
                 for (;;) {
                     npos += pl[j].n;
-                    const bool more = j + 1 < pl.size() && pl[j].n == BUF && pl[j + 1].ts == pl[j].ts + (int64_t)BUF * 5;
+                    const bool more = j + 1 < pl.size() && pl[j].n == BUF && pl[j + 1].ts == pl[j].ts + (int64_t)BUF * 5 && !pl[j + 1].restart;
                     if (!more) break;
                     j++;
                 }
                 const uint32_t nb = (uint32_t)(j - i + 1);
-                add_segment(c, sl, s, region + pl[i].off - (size_t)B200_TRAIL * 2, npos, nb > 1 ? BUF : pl[i].n, nb,
-                            (halo_ok ? 0 : SEG_HALO_ZERO) | (c->kind[s] == 3 ? SEG_MAG : 0), pl[i].ts);
+                add_segment(sl, s, region + pl[i].off - (size_t)B200_TRAIL * 2, npos, nb > 1 ? BUF : pl[i].n, nb,
+                            (halo_ok ? 0 : SEG_HALO_ZERO) | (c->kind[s] == 3 ? SEG_MAG : 0), pl[i].ts, thr);
                 if (c->kind[s] == 3) for (size_t q = i; q <= j; q++) fsum_of_buf.push_back({sl.nbuf - nb + (uint32_t)(q - i), pl[q].fsum});
                 halo_ok = pl[j].n >= B200_TRAIL;      // sdr_ifile.c:209-213
                 i = j + 1;
@@ -872,24 +902,50 @@ API int b200_demod_run(b200_demod_ctx *c) {
     return rc;
 }
 
-static int build_device_run(b200_demod_ctx *c, Slot &sl, const DeviceArgs &a) {
-    const uint32_t S = c->cfg.n_streams, bps = fmt_bytes(a.fmt);
-    if (((uintptr_t)a.d_iq & 15) || (a.stride & 15) || (a.buf_len & 7)) return fail(c, B200_E_INVAL, "d_iq and stream_stride_bytes must be 16-byte aligned and buf_len a multiple of 8");
-    if (a.n_buffers == 0 || a.n_buffers > c->cfg.max_buffers_per_run || a.buf_len == 0 || a.buf_len > c->cfg.buf_samples) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration");
-    if ((uint64_t)a.n_buffers * a.buf_len * bps > a.stride && S > 1) return fail(c, B200_E_INVAL, "stream_stride_bytes smaller than one stream's data");
-    sl.sc16 = a.fmt != FMT_UC8;
-    if (sl.sc16 && !sl.d_slab) {
-        const size_t stride = ((size_t)2 + B200_TRAIL + (size_t)c->cfg.max_buffers_per_run * c->cfg.buf_samples + 32 + 127) & ~(size_t)127;
-        if (dev_alloc(&sl.d_slab, stride * S) != cudaSuccess) { sl.d_slab = nullptr; return fail(c, B200_E_NOMEM, "sc16 magnitude slab (%zu bytes)", stride * S * 2); }
-        sl.slab_stride = stride;
+// Checks a step's arguments before anything is enqueued or changed: `fmt`, the alignment and length rules, every receiver's descriptor and
+// a stride that holds the largest count (*max_n).  `device`: d_iq / stream_stride_bytes must be 16-byte aligned.
+static int check_rx(b200_demod_ctx *c, int fmt, const void *iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx, bool device,
+                    uint32_t *max_n) {
+    const uint32_t S = c->cfg.n_streams;
+    if (!iq || !rx) return fail(c, B200_E_INVAL, "null sample or descriptor pointer");
+    if (fmt != FMT_UC8 && fmt != FMT_SC16 && fmt != FMT_SC16Q11) return fail(c, B200_E_INVAL, "format %d is not B200_FORMAT_UC8, _SC16 or _SC16Q11", fmt);
+    if (device && (((uintptr_t)iq & 15) || (stride & 15))) return fail(c, B200_E_INVAL, "d_iq and stream_stride_bytes must be 16-byte aligned");
+    if (buf_len == 0 || buf_len > c->cfg.buf_samples || (buf_len & 7)) return fail(c, B200_E_INVAL, "buf_len must be 1 .. buf_samples and a multiple of 8");
+    uint32_t m = 0;
+    for (uint32_t s = 0; s < S; s++) {
+        const b200_rx_step &r = rx[s];
+        if (r.n_buffers > c->cfg.max_buffers_per_run) return fail(c, B200_E_INVAL, "receiver %u: %u buffers exceed max_buffers_per_run=%u", s, r.n_buffers, c->cfg.max_buffers_per_run);
+        if (r.preamble_threshold < 0) return fail(c, B200_E_INVAL, "receiver %u: negative preamble threshold", s);
+        if (r.reserved_ || (r.flags & ~B200_RX_CONTINUES)) return fail(c, B200_E_INVAL, "receiver %u: reserved_ and unknown flag bits must be 0", s);
+        m = std::max(m, r.n_buffers);
     }
-    sl.nseg = sl.ntile = sl.nbuf = 0; sl.is_device = true; sl.dargs = a;
+    if ((uint64_t)m * buf_len * fmt_bytes(fmt) > stride && S > 1) return fail(c, B200_E_INVAL, "stride smaller than the largest receiver's data");
+    *max_n = m;
+    return B200_OK;
+}
+
+// Builds a device-resident step in `sl` from checked arguments: one segment per receiver present, none for an absent one.
+static int build_device_run(b200_demod_ctx *c, Slot &sl, int fmt, const uint8_t *d_iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx) {
+    const uint32_t S = c->cfg.n_streams;
+    sl.sc16 = fmt != FMT_UC8;
+    if (sl.sc16 && !sl.d_slab) {
+        const size_t stride16 = ((size_t)2 + B200_TRAIL + (size_t)c->cfg.max_buffers_per_run * c->cfg.buf_samples + 32 + 127) & ~(size_t)127;
+        if (dev_alloc(&sl.d_slab, stride16 * S) != cudaSuccess) { sl.d_slab = nullptr; return fail(c, B200_E_NOMEM, "sc16 magnitude slab (%zu bytes)", stride16 * S * 2); }
+        sl.slab_stride = stride16;
+    }
+    sl.nseg = sl.ntile = sl.nbuf = 0;
+    bool same_counts = sl.cached_counts.size() == S;
+    sl.cached_counts.resize(S);
     for (uint32_t s = 0; s < S; s++) {
         sl.h_stream_seg_begin[s] = sl.nseg;
         sl.stream_buf_begin[s] = sl.nbuf;
-        const uint8_t *base = sl.sc16 ? reinterpret_cast<const uint8_t *>(sl.d_slab + s * sl.slab_stride + 2) : a.d_iq + (size_t)s * a.stride - (size_t)B200_TRAIL * 2;
-        add_segment(c, sl, s, base, a.n_buffers * a.buf_len, a.buf_len, a.n_buffers,
-                    (a.continues ? 0 : SEG_HALO_ZERO) | (sl.sc16 ? SEG_MAG : 0), a.first_ts);
+        const b200_rx_step &r = rx[s];
+        same_counts = same_counts && sl.cached_counts[s] == r.n_buffers;
+        sl.cached_counts[s] = r.n_buffers;
+        if (!r.n_buffers) continue;
+        const uint8_t *base = sl.sc16 ? reinterpret_cast<const uint8_t *>(sl.d_slab + s * sl.slab_stride + 2) : d_iq + (size_t)s * stride - (size_t)B200_TRAIL * 2;
+        add_segment(sl, s, base, r.n_buffers * buf_len, buf_len, r.n_buffers, ((r.flags & B200_RX_CONTINUES) ? 0 : SEG_HALO_ZERO) | (sl.sc16 ? SEG_MAG : 0),
+                    r.first_sample_timestamp, r.preamble_threshold ? r.preamble_threshold : c->cfg.preamble_threshold);
     }
     sl.h_stream_seg_begin[S] = sl.nseg;
     sl.stream_buf_begin[S] = sl.nbuf;
@@ -902,29 +958,44 @@ static int build_device_run(b200_demod_ctx *c, Slot &sl, const DeviceArgs &a) {
     if (sl.sc16) {
         Sc16Params &p = sl.conv;
         p = Sc16Params();
-        p.iq = reinterpret_cast<const uint32_t *>(a.d_iq); p.iq_stride = a.stride / 4;
+        p.iq = reinterpret_cast<const uint32_t *>(d_iq); p.iq_stride = stride / 4;
         p.mag = sl.d_slab + 2; p.mag_stride = sl.slab_stride;
-        p.n_streams = S; p.n_buffers = a.n_buffers; p.buf_len = a.buf_len; p.halo = a.continues ? 1u : 0u;
-        p.scale = a.fmt == FMT_SC16Q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
+        p.n_segs = sl.nseg; p.n_bufs = sl.nbuf; p.buf_len = buf_len;
+        if (sl.nseg) p.seg0 = sl.h_segs[0];
+        p.scale = fmt == FMT_SC16Q11 ? 1.0f / 2048.0f : 1.0f / 32768.0f;
     }
     // the tile -> segment table only depends on the layout; skip its upload when nothing changed
-    const uint64_t key = ((uint64_t)a.n_buffers << 40) ^ ((uint64_t)a.buf_len << 8) ^ (((uintptr_t)a.d_iq >> 4) & 15) ^ (a.stride << 20) ^ ((uint64_t)sl.sc16 << 63);
-    sl.upload_tiles = !(sl.cached_tiles == sl.ntile && sl.cached_layout_key == key);
+    const uint64_t key = ((uint64_t)buf_len << 8) ^ (((uintptr_t)d_iq >> 4) & 15) ^ (stride << 20) ^ ((uint64_t)sl.sc16 << 63);
+    sl.upload_tiles = !(sl.cached_tiles == sl.ntile && sl.cached_layout_key == key && same_counts);
     sl.cached_tiles = sl.ntile; sl.cached_layout_key = key;
     return B200_OK;
+}
+
+// The uniform calls: every receiver delivers n_buffers buffers from first_ts on, all continue or none, the context's threshold.
+static const b200_rx_step *uniform_rx(b200_demod_ctx *c, uint32_t n_buffers, int continues, int64_t first_ts) {
+    for (b200_rx_step &r : c->rx_uniform) { r = b200_rx_step(); r.first_sample_timestamp = first_ts; r.n_buffers = n_buffers; r.flags = continues ? B200_RX_CONTINUES : 0u; }
+    return c->rx_uniform.data();
+}
+
+static int run_device_rx(b200_demod_ctx *c, int fmt, const uint8_t *d_iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx) {
+    if (!c) return B200_E_INVAL;
+    if (any_in_flight(c)) return fail(c, B200_E_STATE, "asynchronous steps are in flight: call b200_demod_wait first");
+    uint32_t max_n;
+    int rc = check_rx(c, fmt, d_iq, stride, buf_len, rx, true, &max_n);
+    if (rc != B200_OK) return rc;
+    CU(c, cudaSetDevice(c->device));
+    Slot &sl = c->slot[0];
+    c->cur = 0;
+    rc = build_device_run(c, sl, fmt, d_iq, stride, buf_len, rx);
+    if (rc != B200_OK) return rc;
+    return execute_blocking(c, sl);
 }
 
 static int run_device(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
                       int continues, int64_t first_ts, int fmt) {
     if (!c || !d_iq) return B200_E_INVAL;
-    if (any_in_flight(c)) return fail(c, B200_E_STATE, "asynchronous steps are in flight: call b200_demod_wait first");
-    CU(c, cudaSetDevice(c->device));
-    Slot &sl = c->slot[0];
-    c->cur = 0;
-    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts, fmt};
-    int rc = build_device_run(c, sl, a);
-    if (rc != B200_OK) return rc;
-    return execute_blocking(c, sl);
+    if (n_buffers == 0) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration");
+    return run_device_rx(c, fmt, d_iq, stride, buf_len, uniform_rx(c, n_buffers, continues, first_ts));
 }
 
 API int b200_demod_run_device_uc8(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
@@ -935,6 +1006,10 @@ API int b200_demod_run_device_uc8(b200_demod_ctx *c, const uint8_t *d_iq, uint64
 API int b200_demod_run_device_sc16(b200_demod_ctx *c, const int16_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
                                    int continues, int64_t first_ts, int q11) {
     return run_device(c, reinterpret_cast<const uint8_t *>(d_iq), stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
+}
+
+API int b200_demod_run_device_rx(b200_demod_ctx *c, int format, const void *d_iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx) {
+    return run_device_rx(c, format, static_cast<const uint8_t *>(d_iq), stride, buf_len, rx);
 }
 
 // ---- asynchronous steps: at most NSLOT in flight ------------------------------------------------------------------------
@@ -950,20 +1025,35 @@ static int launch_async(b200_demod_ctx *c, Slot &sl) {
     return B200_OK;
 }
 
-static int run_device_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
-                            int continues, int64_t first_ts, int fmt) {
-    if (!c || !d_iq) return B200_E_INVAL;
-    CU(c, cudaSetDevice(c->device));
+// The slot the next asynchronous step takes, allocated on first use.
+static int async_slot(b200_demod_ctx *c, Slot **out) {
     Slot &sl = c->slot[c->next_async];
     if (sl.in_flight) return fail(c, B200_E_STATE, "%d steps are already in flight: call b200_demod_wait", NSLOT);
     if (!sl.allocated) {
         cudaError_t e = alloc_slot(c, sl, c->slot[0].rec_cap);
         if (e != cudaSuccess) return fail(c, B200_E_NOMEM, "pipeline slot %d: %s", c->next_async, cudaGetErrorString(e));
     }
-    const DeviceArgs a = {d_iq, stride, n_buffers, buf_len, continues, first_ts, fmt};
-    int rc = build_device_run(c, sl, a);
+    *out = &sl;
+    return B200_OK;
+}
+
+static int run_device_rx_async(b200_demod_ctx *c, int fmt, const uint8_t *d_iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx) {
+    if (!c) return B200_E_INVAL;
+    uint32_t max_n;
+    int rc = check_rx(c, fmt, d_iq, stride, buf_len, rx, true, &max_n);
     if (rc != B200_OK) return rc;
-    return launch_async(c, sl);
+    CU(c, cudaSetDevice(c->device));
+    Slot *sl = nullptr;
+    if ((rc = async_slot(c, &sl)) != B200_OK) return rc;
+    if ((rc = build_device_run(c, *sl, fmt, d_iq, stride, buf_len, rx)) != B200_OK) return rc;
+    return launch_async(c, *sl);
+}
+
+static int run_device_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
+                            int continues, int64_t first_ts, int fmt) {
+    if (!c || !d_iq) return B200_E_INVAL;
+    if (n_buffers == 0) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration");
+    return run_device_rx_async(c, fmt, d_iq, stride, buf_len, uniform_rx(c, n_buffers, continues, first_ts));
 }
 
 API int b200_demod_run_device_uc8_async(b200_demod_ctx *c, const uint8_t *d_iq, uint64_t stride, uint32_t n_buffers, uint32_t buf_len,
@@ -976,29 +1066,31 @@ API int b200_demod_run_device_sc16_async(b200_demod_ctx *c, const int16_t *d_iq,
     return run_device_async(c, reinterpret_cast<const uint8_t *>(d_iq), stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
 }
 
+API int b200_demod_run_device_rx_async(b200_demod_ctx *c, int format, const void *d_iq, uint64_t stride, uint32_t buf_len, const b200_rx_step *rx) {
+    return run_device_rx_async(c, format, static_cast<const uint8_t *>(d_iq), stride, buf_len, rx);
+}
+
 // ---- asynchronous host-buffer steps: the device-resident pipeline fed from library-owned input buffers ----------------
 #define PIPE_LEAD 1024        // bytes in front of each receiver's samples: the 326-sample halo sits right before them
 #define PIPE_LEAD16 2048      // ... for int16 I,Q samples (326 * 4 bytes)
 
-static int run_host_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
-                          int continues, int64_t first_ts, int fmt) {
-    if (!c || !h_iq) return B200_E_INVAL;
+static int run_host_rx_async(b200_demod_ctx *c, int fmt, const uint8_t *h_iq, uint64_t host_stride, uint32_t buf_len, const b200_rx_step *rx) {
+    if (!c) return B200_E_INVAL;
+    uint32_t max_n;
+    int rc = check_rx(c, fmt, h_iq, host_stride, buf_len, rx, false, &max_n);
+    if (rc != B200_OK) return rc;
     CU(c, cudaSetDevice(c->device));
     const uint32_t S = c->cfg.n_streams, K = c->cfg.max_buffers_per_run, BUF = c->cfg.buf_samples, bps = fmt_bytes(fmt);
-    if (n_buffers == 0 || n_buffers > K || buf_len == 0 || buf_len > BUF || (buf_len & 7)) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration (buf_len must be a multiple of 8)");
-    const size_t row = (size_t)n_buffers * buf_len * bps;
-    if (host_stride < row && S > 1) return fail(c, B200_E_INVAL, "host_stride_bytes smaller than one stream's data");
     for (uint32_t s = 0; s < S; s++) if (!c->pending[s].empty()) return fail(c, B200_E_STATE, "buffers submitted for b200_demod_run are pending: run them first");
     const int pi = c->next_async;
-    Slot &sl = c->slot[pi];
-    if (sl.in_flight) return fail(c, B200_E_STATE, "%d steps are already in flight: call b200_demod_wait", NSLOT);
-    if (continues && !(c->pipe_prev_valid && c->pipe_prev_bytes == bps))
-        return fail(c, B200_E_STATE, "continues != 0 but there is no previous %s step with >= 326 samples per receiver",
-                    fmt == FMT_UC8 ? "run_host_uc8_async" : "run_host_sc16_async");
-    if (!sl.allocated) {
-        cudaError_t e = alloc_slot(c, sl, c->slot[0].rec_cap);
-        if (e != cudaSuccess) return fail(c, B200_E_NOMEM, "pipeline slot %d: %s", pi, cudaGetErrorString(e));
-    }
+    if (c->slot[pi].in_flight) return fail(c, B200_E_STATE, "%d steps are already in flight: call b200_demod_wait", NSLOT);
+    for (uint32_t s = 0; s < S; s++)
+        if (rx[s].n_buffers && (rx[s].flags & B200_RX_CONTINUES) && c->halo_bytes[s] != bps)
+            return fail(c, B200_E_STATE, "receiver %u continues, but its last %s step did not leave >= 326 samples", s,
+                        fmt == FMT_UC8 ? "uc8 host-buffer" : "sc16 host-buffer");
+    Slot *slp = nullptr;
+    if ((rc = async_slot(c, &slp)) != B200_OK) return rc;
+    Slot &sl = *slp;
     const size_t lead = fmt == FMT_UC8 ? PIPE_LEAD : PIPE_LEAD16;
     uint8_t **pipe = fmt == FMT_UC8 ? c->d_pipe : c->d_pipe16;
     size_t &pipe_stride = fmt == FMT_UC8 ? c->pipe_stride : c->pipe16_stride;
@@ -1013,21 +1105,41 @@ static int run_host_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_
             if (!c->ev_in[i]) CU(c, cudaEventCreateWithFlags(&c->ev_in[i], cudaEventDisableTiming));
         }
     }
-    // The slot's previous step (NSLOT steps ago) has been collected, so nothing reads pipe[pi] any more; the copies of
-    // consecutive steps are ordered on in_stream, which also orders the halo copy after the previous step's samples.
+    if (!c->d_halo_store) {
+        if (dev_alloc(&c->d_halo_store, (size_t)S * B200_TRAIL * 2) != cudaSuccess || dev_alloc(&c->d_halo_op, (size_t)NSLOT * S) != cudaSuccess ||
+            pin_alloc(&c->h_halo_op, (size_t)NSLOT * S) != cudaSuccess) {
+            cudaFree(c->d_halo_store); cudaFree(c->d_halo_op); cudaFreeHost(c->h_halo_op);
+            c->d_halo_store = nullptr; c->d_halo_op = nullptr; c->h_halo_op = nullptr;
+            return fail(c, B200_E_NOMEM, "halo store of %u receivers", S);
+        }
+    }
     uint8_t *dst = pipe[pi] + lead;
-    const size_t halo = (size_t)B200_TRAIL * bps;
-    CU(c, cudaMemcpy2DAsync(dst, pipe_stride, h_iq, host_stride, row, S, cudaMemcpyHostToDevice, c->in_stream));
-    if (continues)      // the mag_buf overlap copy (sdr_ifile.c:209-213): the previous step's last 326 samples in front of this step's
-        CU(c, cudaMemcpy2DAsync(dst - halo, pipe_stride, pipe[c->pipe_prev] + lead + c->pipe_prev_row - halo, pipe_stride,
-                                halo, S, cudaMemcpyDeviceToDevice, c->in_stream));
+    if ((rc = build_device_run(c, sl, fmt, dst, pipe_stride, buf_len, rx)) != B200_OK) return rc;
+    // The slot's previous step (NSLOT steps ago) has been collected, so nothing reads pipe[pi] or this slot's halo_op any more; the
+    // copies and halo_store_kernel of consecutive steps are ordered on in_stream, so a receiver's stored halo is the one its last
+    // step left.
+    sl.cached_tiles = 0;                  // (until the step is enqueued: a failure below leaves no valid tile table behind)
+    const size_t row = (size_t)max_n * buf_len * bps;
+    if (row) CU(c, cudaMemcpy2DAsync(dst, pipe_stride, h_iq, host_stride, row, S, cudaMemcpyHostToDevice, c->in_stream));
+    uint32_t *op = c->h_halo_op + (size_t)pi * S;
+    for (uint32_t s = 0; s < S; s++)
+        op[s] = rx[s].n_buffers ? (rx[s].n_buffers * buf_len) << 1 | ((rx[s].flags & B200_RX_CONTINUES) ? 1u : 0u) : 0u;
+    CU(c, cudaMemcpyAsync(c->d_halo_op + (size_t)pi * S, op, (size_t)S * 4, cudaMemcpyHostToDevice, c->in_stream));
+    halo_store_kernel<<<S, 128, 0, c->in_stream>>>(dst, pipe_stride, c->d_halo_store, c->d_halo_op + (size_t)pi * S, bps);
+    CU(c, cudaGetLastError());
     CU(c, cudaEventRecord(c->ev_in[pi], c->in_stream));
     CU(c, cudaStreamWaitEvent(c->stream, c->ev_in[pi], 0));
-    c->pipe_prev = pi; c->pipe_prev_row = row; c->pipe_prev_valid = row >= halo; c->pipe_prev_bytes = bps;
-    const DeviceArgs a = {dst, pipe_stride, n_buffers, buf_len, continues ? 1 : 0, first_ts, fmt};
-    int rc = build_device_run(c, sl, a);
-    if (rc != B200_OK) return rc;
+    for (uint32_t s = 0; s < S; s++)
+        if (rx[s].n_buffers) c->halo_bytes[s] = rx[s].n_buffers * buf_len >= B200_TRAIL ? (uint8_t)bps : 0;
+    sl.cached_tiles = sl.ntile;
     return launch_async(c, sl);
+}
+
+static int run_host_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
+                          int continues, int64_t first_ts, int fmt) {
+    if (!c || !h_iq) return B200_E_INVAL;
+    if (n_buffers == 0) return fail(c, B200_E_INVAL, "n_buffers/buf_len exceed the context's configuration (buf_len must be a multiple of 8)");
+    return run_host_rx_async(c, fmt, h_iq, host_stride, buf_len, uniform_rx(c, n_buffers, continues, first_ts));
 }
 
 API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
@@ -1038,6 +1150,10 @@ API int b200_demod_run_host_uc8_async(b200_demod_ctx *c, const uint8_t *h_iq, ui
 API int b200_demod_run_host_sc16_async(b200_demod_ctx *c, const int16_t *h_iq, uint64_t host_stride, uint32_t n_buffers, uint32_t buf_len,
                                        int continues, int64_t first_ts, int q11) {
     return run_host_async(c, reinterpret_cast<const uint8_t *>(h_iq), host_stride, n_buffers, buf_len, continues, first_ts, q11 ? FMT_SC16Q11 : FMT_SC16);
+}
+
+API int b200_demod_run_host_rx_async(b200_demod_ctx *c, int format, const void *h_iq, uint64_t host_stride, uint32_t buf_len, const b200_rx_step *rx) {
+    return run_host_rx_async(c, format, static_cast<const uint8_t *>(h_iq), host_stride, buf_len, rx);
 }
 
 // Pipelined steps keep three kernels' worth of work in flight: the scan of step n+1 (one persistent CTA per SM, the whole SM each)

@@ -523,7 +523,7 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
             const uint32_t e = b0 + lane;
             if (e < n_q1) {
                 pl = (Q1_SMEM >= CHUNK || e < Q1_SMEM) ? W.q1[e] : W_Q1_OVER(W, P)[e - Q1_SMEM];      // chunk-local position
-                tried = threshold_phases(mag0 + pl, P.thr);
+                tried = threshold_phases(mag0 + pl, reinterpret_cast<const Segment *>(W.seg)->thr);     // the receiver's own threshold
             }
             bal = __ballot_sync(FULLMASK, tried != 0);
         }

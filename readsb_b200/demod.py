@@ -13,7 +13,7 @@ from pathlib import Path
 
 import numpy as np
 
-from .abi import BUFRES_DTYPE, CFG_MODE_AC, CFG_NO_TIMING, FRAME_DTYPE, MODEAC_DTYPE, Config, Stats
+from .abi import BUFRES_DTYPE, CFG_MODE_AC, CFG_NO_TIMING, FRAME_DTYPE, MODEAC_DTYPE, RX_STEP_DTYPE, Config, Stats
 
 _LIB = None
 LIB_PATH = Path(__file__).resolve().parent / "libb200demod.so"
@@ -57,6 +57,10 @@ def lib():
         L.b200_demod_run_device_sc16.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
         L.b200_demod_run_device_sc16_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
         L.b200_demod_run_host_sc16_async.argtypes = [vp, vp, u64, u32, u32, C.c_int, i64, C.c_int]
+        L.b200_demod_run_device_rx.argtypes = [vp, C.c_int, vp, u64, u32, vp]
+        L.b200_demod_run_device_rx_async.argtypes = [vp, C.c_int, vp, u64, u32, vp]
+        L.b200_demod_run_host_rx_async.argtypes = [vp, C.c_int, vp, u64, u32, vp]
+        L.b200_demod_restart_stream.argtypes = [vp, u32]
         L.b200_demod_wait.argtypes = [vp]
         L.b200_demod_frame_count.argtypes = [vp, u32, C.POINTER(u32)]
         L.b200_demod_fetch.argtypes = [vp, u32, vp, u32, C.POINTER(u32)]
@@ -87,6 +91,7 @@ EXPORTED_SYMBOLS = [
     "b200_demod_run_device_uc8_async", "b200_demod_wait", "b200_demod_fetch_modeac", "b200_demod_run_host_uc8_async",
     "b200_demod_submit_mag_u16_levels", "b200_demod_set_preamble_threshold",
     "b200_demod_run_device_sc16", "b200_demod_run_device_sc16_async", "b200_demod_run_host_sc16_async",
+    "b200_demod_run_device_rx", "b200_demod_run_device_rx_async", "b200_demod_run_host_rx_async", "b200_demod_restart_stream",
 ]
 
 
@@ -214,6 +219,28 @@ class Demodulator:
                             first_sample_timestamp: int, q11: bool = False):
         self._check(self.L.b200_demod_run_host_sc16_async(self.h, h_ptr, host_stride_bytes, n_buffers, buf_len,
                                                           1 if continues else 0, first_sample_timestamp, 1 if q11 else 0))
+
+    # -- independent receivers: one b200_rx_step per receiver (abi.RX_STEP_DTYPE), format abi.FORMAT_* ---------------------
+    def _rx(self, rx: np.ndarray):
+        rx = np.ascontiguousarray(rx, dtype=RX_STEP_DTYPE)
+        assert rx.shape == (self.n_streams,), "one descriptor per receiver of the context"
+        return rx
+
+    def run_device_rx(self, fmt: int, d_ptr: int, stream_stride_bytes: int, buf_len: int, rx: np.ndarray):
+        rx = self._rx(rx)
+        self._check(self.L.b200_demod_run_device_rx(self.h, fmt, d_ptr, stream_stride_bytes, buf_len, rx.ctypes.data))
+
+    def run_device_rx_async(self, fmt: int, d_ptr: int, stream_stride_bytes: int, buf_len: int, rx: np.ndarray):
+        rx = self._rx(rx)
+        self._check(self.L.b200_demod_run_device_rx_async(self.h, fmt, d_ptr, stream_stride_bytes, buf_len, rx.ctypes.data))
+
+    def run_host_rx_async(self, fmt: int, h_ptr: int, host_stride_bytes: int, buf_len: int, rx: np.ndarray):
+        rx = self._rx(rx)
+        self._check(self.L.b200_demod_run_host_rx_async(self.h, fmt, h_ptr, host_stride_bytes, buf_len, rx.ctypes.data))
+
+    def restart_stream(self, stream: int):
+        """The receiver's next submit_iq* buffer starts with a zero halo (a block was dropped in front of it)."""
+        self._check(self.L.b200_demod_restart_stream(self.h, stream))
 
     def wait(self):
         self._check(self.L.b200_demod_wait(self.h))

@@ -6,7 +6,7 @@ Each case draws: receivers, buffer length (odd sizes included), buffers per run,
 saturated / sawtooth / constant / uniformly random bytes), preamble threshold, --no-fix / --no-fix-df, Mode A/C on or off, the
 ICAO filter's flip period (down to a few ms of stream time: flips inside a run), a ragged tail, and one of the entry paths
 (host submits, magnitude hand-off, sc16 / sc16q11 input, device-resident blocking, device-resident pipelined, pipelined host
-slab).  Frames, per-buffer results, counters, Mode A/C replies and (sometimes) the Beast byte stream must equal the oracle's.
+slab, or independent receivers through the _rx calls with their own counts, restarts and thresholds).  Frames, per-buffer results, counters, Mode A/C replies and (sometimes) the Beast byte stream must equal the oracle's.
 Prints the failing case's parameters (re-run it alone with --only K).  The same script works on a GPU (without B200_EMU).
 """
 from __future__ import annotations
@@ -68,7 +68,7 @@ def to_sc16(iq8, q11: bool, seed: int):
     return np.clip(v, -2048 if q11 else -32768, 2047 if q11 else 32767).astype(np.int16)
 
 
-def run_case(k: int, seed: int, verbose: bool):
+def run_case(k: int, seed: int, verbose: bool, only_path: str | None = None):
     import numpy as np
     import devbuf
     from oraclelib import Oracle
@@ -77,7 +77,8 @@ def run_case(k: int, seed: int, verbose: bool):
     rng = np.random.default_rng([seed, k])
     S = int(rng.choice([1, 1, 2, 3, 5]))
     buf = int(rng.choice([1000, 4096, 8191, 8192, 20000, 32768, 65536, 65536, 131072, int(rng.integers(700, 70000))]))
-    path = str(rng.choice(["host", "host", "mag", "device", "device_async", "host_async", "sc16", "host_var", "mixed", "host_ops"]))
+    path = str(rng.choice(["host", "host", "mag", "device", "device_async", "host_async", "sc16", "host_var", "mixed", "host_ops", "rx"]))
+    path = only_path or path
     if path in ("device", "device_async", "host_async"):
         buf = max(8, buf & ~7)                                   # those entry points want multiples of 8
     K = int(rng.choice([1, 2, 3, 4, 8]))
@@ -184,6 +185,16 @@ def run_case(k: int, seed: int, verbose: bool):
             problems += [f"stream {s_}: {p}" for p in diff_frames(np.concatenate(gf[s_]), np.concatenate(of[s_])) + diff_stats(d.stats(s_), oracles[s_].stats())]
         d.close()
         return params, problems, sum(len(np.concatenate(x)) for x in gf)
+    if path == "rx":            # independent receivers: per-receiver counts (0 included), clock gaps with restarts, thresholds 0 / 40 / 75
+        from test_gpu_rx_steps import FORMATS, _Session
+        d.close()
+        sess = _Session(str(rng.choice(["device", "device_async", "host"])), int(rng.choice(FORMATS)), S=S, K=K, buf=max(8, buf & ~7), steps=max(steps, 2),
+                        depth=int(rng.choice([2, 3])), ttl=ttl, mode_ac=mode_ac, seed=int(rng.integers(1 << 30)))
+        params.update(rx_path=sess.path, fmt=sess.fmt, plan=sess.plan)
+        try:
+            return params, [], sess.run().check(min_frames=0)
+        except AssertionError as e:
+            return params, [str(e)[:2000]], 0
     if path == "mixed":         # every receiver its own entry point and its own amount of data, all in the same runs
         kinds = [str(rng.choice(["host", "mag", "sc16"])) for _ in range(S)]
         tot = [int(max(1, total * rng.uniform(0.2, 1.0))) for _ in range(S)]
@@ -378,6 +389,7 @@ def main():
     ap.add_argument("--minutes", type=float, default=0.0, help="stop after this many minutes (0 = run all cases)")
     ap.add_argument("--only", type=int, default=-1)
     ap.add_argument("--emu", type=int, default=1, help="1: the emulated library (default), 0: the sm_90a library on a GPU")
+    ap.add_argument("--path", help="every case on this entry path (the other draws stay as they are)")
     ap.add_argument("-v", action="store_true")
     a = ap.parse_args()
     if a.emu:
@@ -388,7 +400,7 @@ def main():
     t0, bad, frames = time.time(), 0, 0
     ks = [a.only] if a.only >= 0 else range(a.cases)
     for k in ks:
-        params, problems, nf = run_case(k, a.seed, a.v)
+        params, problems, nf = run_case(k, a.seed, a.v, a.path)
         frames += nf
         if problems:
             bad += 1
