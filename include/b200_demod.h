@@ -294,8 +294,9 @@ enum { B200_FORMAT_UC8 = 0, B200_FORMAT_SC16 = 1, B200_FORMAT_SC16Q11 = 2 };
  *     samples_dropped is non-zero); 0 = the context's.
  * Refused with B200_E_INVAL before anything is enqueued or changed (no halo stored, no pipeline slot taken): a bad format, n_buffers
  * above max_buffers_per_run, a negative threshold, non-zero reserved_ or unknown flag bits, a stride too small for the largest count,
- * and the alignment / buf_len rules.  Results, waits and pipelining as for the calls above; the uniform calls are these calls with
- * one descriptor repeated. */
+ * the alignment / buf_len rules, and buffers shorter than the 326-sample halo other than one per step without B200_RX_CONTINUES (the
+ * reference gives the buffer after a short one a zero halo, sdr_ifile.c:207-212).  Results, waits and pipelining as for the calls
+ * above; the uniform calls are these calls with one descriptor repeated. */
 int b200_demod_run_device_rx(b200_demod_ctx *ctx, int format, const void *d_iq, uint64_t stream_stride_bytes, uint32_t buf_len,
                              const b200_rx_step *rx);
 int b200_demod_run_device_rx_async(b200_demod_ctx *ctx, int format, const void *d_iq, uint64_t stream_stride_bytes, uint32_t buf_len,

@@ -839,7 +839,8 @@ API int b200_demod_run(b200_demod_ctx *c) {
                 add_segment(sl, s, region + p.off, p.n, p.n, 1, SEG_MAG, p.ts, thr);
             }
         } else {
-            // consecutive full buffers with contiguous timestamps form one segment; a partial buffer ends it
+            // consecutive full buffers with contiguous timestamps form one segment; a partial buffer ends it, and so does every buffer
+            // shorter than the halo: the buffer after it starts with a zero halo (sdr_ifile.c:207-212), not with its samples
             size_t i = 0;
             bool halo_ok = c->halo_valid[s];
             while (i < pl.size()) {
@@ -848,7 +849,7 @@ API int b200_demod_run(b200_demod_ctx *c) {
                 if (pl[i].restart) halo_ok = false;        // sdr_rtlsdr.c:381-385: a buffer after dropped samples starts with a zero halo
                 for (;;) {
                     npos += pl[j].n;
-                    const bool more = j + 1 < pl.size() && pl[j].n == BUF && pl[j + 1].ts == pl[j].ts + (int64_t)BUF * 5 && !pl[j + 1].restart;
+                    const bool more = j + 1 < pl.size() && pl[j].n == BUF && BUF >= B200_TRAIL && pl[j + 1].ts == pl[j].ts + (int64_t)BUF * 5 && !pl[j + 1].restart;
                     if (!more) break;
                     j++;
                 }
@@ -918,6 +919,9 @@ static int check_rx(b200_demod_ctx *c, int fmt, const void *iq, uint64_t stride,
         if (r.preamble_threshold < 0) return fail(c, B200_E_INVAL, "receiver %u: negative preamble threshold", s);
         if (r.reserved_ || (r.flags & ~B200_RX_CONTINUES)) return fail(c, B200_E_INVAL, "receiver %u: reserved_ and unknown flag bits must be 0", s);
         m = std::max(m, r.n_buffers);
+        // a buffer shorter than the halo leaves the next one a zero halo (sdr_ifile.c:207-212), which a step's segment cannot express
+        if (buf_len < B200_TRAIL && (r.n_buffers > 1 || (r.n_buffers && (r.flags & B200_RX_CONTINUES))))
+            return fail(c, B200_E_INVAL, "receiver %u: buffers of %u < %u samples go one per step, without B200_RX_CONTINUES", s, buf_len, (unsigned)B200_TRAIL);
     }
     if ((uint64_t)m * buf_len * fmt_bytes(fmt) > stride && S > 1) return fail(c, B200_E_INVAL, "stride smaller than the largest receiver's data");
     *max_n = m;

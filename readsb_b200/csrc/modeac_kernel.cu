@@ -94,6 +94,14 @@ __device__ __forceinline__ uint32_t ac_bits(const M &m, uint32_t j, uint32_t noi
 }
 
 // ---- noise floor per reference buffer --------------------------------------------------------------------------------
+// `(unsigned)x` of the reference's noise floor as its x86-64 build evaluates it: gcc converts a double to a 32-bit unsigned
+// through the 64-bit cvttsd2si, so the floor wraps modulo 2^32 below 2^63 and is 0 for NaN and beyond (0x8000000000000000
+// truncated).  cvt.rzi.u32.f64 would clamp at 0xffffffff instead.  (An aarch64 build of the reference clamps too.)  The
+// floor is never negative: the square root is NaN unless mean_power >= mean_level^2 >= 0.
+__device__ __forceinline__ uint32_t u32_of_double_x86(double x) {
+    return (x >= 0.0 && x < 9223372036854775808.0) ? (uint32_t)(uint64_t)x : 0u;
+}
+
 __global__ void modeac_noise_kernel(const AcScanParams P) {
     for (uint32_t si = blockIdx.x; si < P.n_segs; si += gridDim.x) {
         const Segment seg = P.segs[si];
@@ -112,7 +120,7 @@ __global__ void modeac_noise_kernel(const AcScanParams P) {
                 mean_power = (double)a.sum_power / 65535.0 / 65535.0 / (double)len;  // convert.c:104-106
             }
             const double noise_stddev = sqrt(mean_power - mean_level * mean_level);           // demod_2400.c:580
-            P.noise[seg.first_buf + b] = (uint32_t)((mean_power + noise_stddev) * 65535 + 0.5);   // :581
+            P.noise[seg.first_buf + b] = u32_of_double_x86((mean_power + noise_stddev) * 65535 + 0.5);   // :581
         }
     }
 }
