@@ -39,24 +39,21 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found: the CUDA library cannot be built")
 
 
-def build_demod(force: bool = False, verbose: bool = False, defines=(), out: Path | None = None) -> Path:
-    """defines / out: an experimental variant of the library (-D macros of csrc/*.cu) next to the product one; selected at
-    run time with B200_DEMOD_LIB=<path> (readsb_b200/demod.py), used by tools/ for A/B timing on the GPU."""
+def build_demod(force: bool = False, verbose: bool = False) -> Path:
     srcs = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) \
         + [ROOT / "include" / "b200_demod.h"]
-    target = out or LIB_DEMOD
-    if not force and _newer(target, srcs):
-        return target
-    cmd = [_nvcc(), *NVCC_FLAGS, "-I", str(ROOT / "include"), "-I", str(CSRC)] + [f"-D{d}" for d in defines]
+    if not force and _newer(LIB_DEMOD, srcs):
+        return LIB_DEMOD
+    cmd = [_nvcc(), *NVCC_FLAGS, "-I", str(ROOT / "include"), "-I", str(CSRC)]
     if verbose:
         cmd += ["-Xptxas", "-v"]
-    cmd += [str(s) for s in sorted(CSRC.glob("*.cu"))] + ["-o", str(target)]
+    cmd += [str(s) for s in sorted(CSRC.glob("*.cu"))] + ["-o", str(LIB_DEMOD)]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)
     if verbose:
         print(res.stderr)
-    return target
+    return LIB_DEMOD
 
 
 def build_synth(force: bool = False) -> Path:

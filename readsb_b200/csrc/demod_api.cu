@@ -384,9 +384,8 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
         // the small finalize CTAs fit next to them.
         int prio_lo = 0, prio_hi = 0;
         CUC(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-        const bool scan_first = getenv("B200_SCAN_PRIO") != nullptr;        // experiment knob (tools/gpu_partition.sh): the scan's stream gets the high priority
-        CUC(cudaStreamCreateWithPriority(&c->own_stream, cudaStreamNonBlocking, scan_first ? prio_hi : prio_lo));
-        CUC(cudaStreamCreateWithPriority(&c->res_stream, cudaStreamNonBlocking, scan_first ? prio_lo : prio_hi));
+        CUC(cudaStreamCreateWithPriority(&c->own_stream, cudaStreamNonBlocking, prio_lo));
+        CUC(cudaStreamCreateWithPriority(&c->res_stream, cudaStreamNonBlocking, prio_hi));
         CUC(cudaStreamCreateWithPriority(&c->copy_stream, cudaStreamNonBlocking, prio_lo));
         CUC(cudaStreamCreateWithPriority(&c->in_stream, cudaStreamNonBlocking, prio_lo));
     }
@@ -1365,10 +1364,6 @@ API int b200_demod_debug_counters(b200_demod_ctx *c, uint64_t out[8]) {
     out[5] = sl.nseg; out[6] = sl.nbuf; out[7] = sl.run_frames;
     return B200_OK;
 }
-
-#ifdef B200_SOLO_CLOCKS
-API int b200_demod_debug_ctl(b200_demod_ctx *c, uint32_t out[8]) { memcpy(out, c->slot[c->cur].h_ctl, 32); return B200_OK; }
-#endif
 
 // ---- ICAO filter control -------------------------------------------------------------------------
 static int icao_op(b200_demod_ctx *c, uint32_t s, int op, uint32_t addr, int *result) {

@@ -28,9 +28,7 @@ __device__ __forceinline__ void uc8_pair_to_mag(const uint16_t *lut_smem, uint32
     const uint32_t sgn = prmt(w, 0, 0xba98);                // 0xff where the byte is >= 128
     const uint32_t f = (w ^ sgn) & 0x7f7f7f7fu;             // fold: v>=128 ? 255-v : v  (127 = centre, 0 = full scale; one LOP3)
     uint32_t off = f + (f & 0x007f007fu);                   // per half: fq*256 + 2*fi
-#ifndef LUT_NO_SWIZZLE                                       // (experiment knob, tools/gpu_variants.sh: two ALU operations less per sample pair, more bank conflicts)
     off ^= (f >> 5) & 0x00780078u;                          // bank swizzle
-#endif
     m0 = *reinterpret_cast<const uint16_t *>(reinterpret_cast<const uint8_t *>(lut_smem) + (off & 0xffffu));
     m1 = *reinterpret_cast<const uint16_t *>(reinterpret_cast<const uint8_t *>(lut_smem) + (off >> 16));
 }

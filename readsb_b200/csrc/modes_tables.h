@@ -47,11 +47,7 @@ static inline uint32_t b200_crc32_ieee(const void *data, size_t n) {
 static inline void b200_build_folded_lut(const uint16_t *lut_full, uint16_t *fold) {
     for (int fq = 0; fq < 128; fq++)
         for (int fi = 0; fi < 128; fi++)
-#ifndef LUT_NO_SWIZZLE
             fold[fq * 128 + (fi ^ ((fq & 15) << 2))] = lut_full[fi * 256 + fq];
-#else
-            fold[fq * 128 + fi] = lut_full[fi * 256 + fq];
-#endif
 }
 
 static inline uint32_t b200_crc24_bytes(const uint32_t *tab, const uint8_t *msg, int nbytes) {

@@ -235,7 +235,6 @@ __device__ __forceinline__ void resolve_buffer(const bool DEFER, const ResolvePa
 
         // score every tried phase with the current filter; first strictly greatest wins (demod_2400.c:243)
         int best = -2; uint32_t best_rel = 0, best_phase = 0, best_key = 0; bool best_known = false;
-#ifndef RESOLVE_PER_POSITION
         // The chunk's records (about one for every two positions) are scored ONE PER LANE in a single pass; then every position
         // picks its own (at most five, consecutive, in phase order) with shuffles.  Scoring per position instead walks the five
         // phases with two or three lanes active each.  More than 32 records in a chunk: further rounds.
@@ -262,21 +261,6 @@ __device__ __forceinline__ void resolve_buffer(const bool DEFER, const ResolvePa
                 }
             }
         }
-#else   // the earlier form, kept for A/B timing (tools/gpu_variants.sh): every position walks its own phases
-        if (valid && live) {
-            uint32_t k = rec_rel + rprefix;
-#pragma unroll
-            for (uint32_t ph = 0; ph < 5; ph++) {
-                if ((live >> ph) & 1u) {
-                    const uint32_t key = key_ptr[k];
-                    const bool known = known_addr(key & 0xffffffu);
-                    const int sc = rec_score((key >> 24) & 7u, known);
-                    if (sc > best) { best = sc; best_rel = k; best_phase = ph; best_key = key; best_known = known; }
-                    k++;
-                }
-            }
-        }
-#endif
         // accept test of decodeModesMessage (mode_s.c:443-596): only a corrected AA that is unknown rejects
         const bool decode_ok = best >= 0 && !((best_key & KEY_AA_CHANGED) && !best_known);
         // Commit the chunk in order.  After an accept the skip-ahead (demod_2400.c:468) silently consumes the
@@ -394,14 +378,6 @@ __device__ __noinline__ void resolve_buffer_call(bool defer, const ResolveParams
     resolve_buffer<BIG>(defer, P, S, R, out, seg, si, b, d_lo, d_hi, skip_in, seq, F, fout, fcap, lane);
 }
 
-#ifdef B200_SOLO_CLOCKS      // analysis build only (tools/gpu_latency.py): where the one-receiver kernel's microseconds go
-__device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-__device__ unsigned long long g_solo_t[8];
-#define SOLO_T(i) do { if (COMPACT && threadIdx.x == 0) g_solo_t[i] = gtime(); } while (0)
-#else
-#define SOLO_T(i) do { } while (0)
-#endif
-
 // COMPACT (the one-receiver kernel): the capacity check (capacity_check_all) is made here, by the CTA itself, while the other
 // threads already fetch the tables.  *n_frames_out (shared memory) receives the receiver's frame count, or ~0 when stage B must not run.
 template <bool BIG, bool COMPACT>
@@ -464,7 +440,6 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
     }
     __syncthreads();
 
-    SOLO_T(1);
     // state only warp 0 touches (the commit step)
     uint32_t armed = st->flip_armed, seq = st->buffer_seq;
     int64_t next_flip = st->next_flip_ms;
@@ -508,7 +483,6 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
                                          fstream + cap_base + (size_t)wid * ucap, ucap_fit, lane);
             }
             __syncthreads();
-            SOLO_T(2);
             // ---- commit, in order -----------------------------------------------------------------------------------------------
             if (wid == 0) {
                 bool spec_ok = true;
@@ -614,7 +588,6 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
         }
     }
 
-    SOLO_T(3);
     // write back
     if (wid == 0) {
         const uint32_t active = s_active;
@@ -699,9 +672,7 @@ __device__ __forceinline__ bool stage_b_runs(const ResolveParams &P) {
 
 // Receivers with grown tables (BIG) are rare: they get an instantiation of their own, launched only when there is one, so that
 // the common case does not share its register allocation; each CTA of either launch leaves the other kind alone.
-#ifndef RS_MIN_CTAS
 #define RS_MIN_CTAS 2         // CTAs per SM the register allocation aims at (128 registers; 3 -> 85: see DESIGN.md 6, SM partition experiment)
-#endif
 template <bool BIG>
 __global__ void __launch_bounds__(RS_WARPS * 32, RS_MIN_CTAS) resolve_kernel(const ResolveParams P) {
     extern __shared__ uint4 resolve_smem_raw[];
@@ -740,18 +711,11 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
     const uint32_t stream = 0;
     StreamState *st = &P.state[0];
     __shared__ uint32_t s_nframes;
-#ifdef B200_SOLO_CLOCKS
-    if (threadIdx.x == 0) g_solo_t[0] = gtime();
-#endif
     if (st->cap_log2 == ICAO_CAP_LOG2) resolve_stream<false, true>(P, S, st, stream, &s_nframes);
     else resolve_stream_big(P, S, st, stream, &s_nframes);
     __syncthreads();
     const uint32_t n = s_nframes == ~0u ? 0u : s_nframes;         // ~0: stage B did not run (the step is going to be repeated)
     if (threadIdx.x == 0) { P.fin.frame_span[0] = 0; P.fin.frame_span[1] = n; P.ctl->total_frames = n; }
-#ifdef B200_SOLO_CLOCKS
-    __syncthreads();
-    if (threadIdx.x == 0) g_solo_t[4] = gtime();
-#endif
     finalize_stream(P.fin, stream, 0, n, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
     if (P.carry_src && s_nframes != ~0u) {      // (not when the step is going to be repeated: it needs its halo again) every reader of this
                                                 // run's samples - scan kernel, finalizer above - is done: move the tail to the front
@@ -766,15 +730,6 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
         uint4 *clr = const_cast<uint4 *>(P.publish_src);
         for (uint32_t i = threadIdx.x; i < P.publish_clear / 16; i += blockDim.x) clr[i] = make_uint4(0, 0, 0, 0);
     }
-#ifdef B200_SOLO_CLOCKS
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        g_solo_t[5] = gtime();
-        P.ctl->pad0_ = (uint32_t)(g_solo_t[1] - g_solo_t[0]); P.ctl->pad_[0] = (uint32_t)(g_solo_t[2] - g_solo_t[1]);
-        P.ctl->pad_[1] = (uint32_t)(g_solo_t[3] - g_solo_t[2]); P.ctl->stage_need = (uint32_t)(g_solo_t[4] - g_solo_t[3]);
-        P.ctl->rec_alloc = (uint32_t)(g_solo_t[5] - g_solo_t[4]);
-    }
-#endif
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -38,17 +38,11 @@ extern "C" { __attribute__((visibility("default"))) unsigned long long b200_scan
 enum { SCN_RUNS, SCN_LOOP_ITERS, SCN_WINDOW_CHUNKS, SCN_FAST_CONVERTS, SCN_EDGE_CONVERTS, SCN_Q1_ENTRIES, SCN_Q1_LOOP_TRIPS, SCN_THR_BATCHES,
        SCN_PASS_BATCHES, SCN_PASSERS, SCN_GATE_TRIPS, SCN_SURVIVORS, SCN_SLICE_ROUNDS, SCN_SLICE_BYTES };
 
-#ifndef SC_WARPS
 #define SC_WARPS 28
-#endif
-#ifndef SC_MAXNREG
-#define SC_MAXNREG 72                         // SC_WARPS x 32 x SC_MAXNREG <= 65536 registers per SM (tools/gpu_variants.sh times other splits)
-#endif
+#define SC_MAXNREG 72                         // SC_WARPS x 32 x SC_MAXNREG <= 65536 registers per SM (other splits were slower: DESIGN.md §4, "Tried and NOT in the code")
 #define CHUNK 512
 #define TILE_CHUNKS (SCAN_TILE / CHUNK)       // 4 chunks of positions per tile
-#ifndef RUN_MAX
 #define RUN_MAX 8                             // a warp takes runs of up to 8 consecutive tiles of one segment (guided self-scheduling)
-#endif
 #define RUN_CHUNKS_MAX (RUN_MAX * TILE_CHUNKS)
 #define MAG_RING (3 * CHUNK)
 #define MAG_MIRROR 64                         // first samples of slot 0 again behind slot 2: reads never wrap
@@ -56,9 +50,7 @@ enum { SCN_RUNS, SCN_LOOP_ITERS, SCN_WINDOW_CHUNKS, SCN_FAST_CONVERTS, SCN_EDGE_
 #define TICK_BITS (5 * CHUNK)
 #define TICK_RING (2 * TICK_CW)
 #define TICK_MIRROR 12
-#ifndef Q1_SMEM
 #define Q1_SMEM 128                           // pre-check passers of a chunk kept in shared memory (58 on receiver noise); the rest (dense input) spills to global memory
-#endif
 #define SURV_CAP 64
 #define TICKG_WORDS ((RUN_CHUNKS_MAX + 1) * TICK_CW + 8)   // per-warp global copy of a whole run's ticks (slicing is deferred and pooled)
 
@@ -102,9 +94,9 @@ struct ScanSmem {                             // the read-only tables every warp
     uint32_t pad_[3];
 };
 
-template <int NW> struct ScanSmemFull {
+struct ScanSmemFull {
     ScanSmem t;
-    WarpSmem w[NW];
+    WarpSmem w[SC_WARPS];
 };
 
 __device__ __forceinline__ void stg_keep(uint32_t *p, uint32_t v, unsigned long long policy) {
@@ -522,7 +514,7 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
             SCAN_COUNT(SCN_THR_BATCHES, 1);
             const uint32_t e = b0 + lane;
             if (e < n_q1) {
-                pl = (Q1_SMEM >= CHUNK || e < Q1_SMEM) ? W.q1[e] : W_Q1_OVER(W, P)[e - Q1_SMEM];      // chunk-local position
+                pl = e < Q1_SMEM ? W.q1[e] : W_Q1_OVER(W, P)[e - Q1_SMEM];      // chunk-local position
                 tried = threshold_phases(mag0 + pl, reinterpret_cast<const Segment *>(W.seg)->thr);     // the receiver's own threshold
             }
             bal = __ballot_sync(FULLMASK, tried != 0);
@@ -639,11 +631,11 @@ __device__ __noinline__ void finish_shared_tile(WarpSmem &W0, WarpSmem &W, const
 // SUB: the launcher's small-run form, a tile shared between the warps of its CTA (finish_shared_tile).  KEEP: a Mode A/C context, the
 // magnitudes are also written to ScanParams::mag_copy.  Both are compile-time so that the plain kernel - the one the throughput is
 // measured on - carries nothing of either (measured with them as run-time tests: 4 - 6 % slower).
-template <int NW, bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kernel(const __grid_constant__ ScanParams P, const DeviceTables *__restrict__ tables) {
+template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kernel(const __grid_constant__ ScanParams P, const DeviceTables *__restrict__ tables) {
     const uint32_t sub_chunks = SUB ? P.sub_chunks : 0u;
-    constexpr uint32_t SC_THREADS = NW * 32;
+    constexpr uint32_t SC_THREADS = SC_WARPS * 32;
     extern __shared__ uint4 smem_raw[];
-    ScanSmemFull<NW> &F = *reinterpret_cast<ScanSmemFull<NW> *>(smem_raw);
+    ScanSmemFull &F = *reinterpret_cast<ScanSmemFull *>(smem_raw);
     ScanSmem &S = F.t;
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 
@@ -811,7 +803,7 @@ template <int NW, bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) s
 #endif
                 while (mb) {
                     const uint32_t b = __ffs(mb) - 1; mb &= mb - 1;
-                    if (Q1_SMEM >= CHUNK || off < Q1_SMEM) W.q1[off] = (uint16_t)(i0 + b); else W_Q1_OVER(W, P)[off - Q1_SMEM] = (uint16_t)(i0 + b);
+                    if (off < Q1_SMEM) W.q1[off] = (uint16_t)(i0 + b); else W_Q1_OVER(W, P)[off - Q1_SMEM] = (uint16_t)(i0 + b);
                     off++;
                 }
                 ms = ms == 2 ? 0 : ms + 1;
@@ -857,35 +849,32 @@ extern "C" int b200_scan_tick_words(void) { return TICKG_WORDS; }
 
 // Kernel attributes are per device: b200_demod_create calls this for the context's device (current at that point).
 extern "C" int b200_prepare_scan(void) {
-    const int bytes = (int)sizeof(ScanSmemFull<SC_WARPS>);
-    cudaError_t e = cudaFuncSetAttribute(scan_kernel<SC_WARPS, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<SC_WARPS, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<SC_WARPS, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<SC_WARPS, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    const int bytes = (int)sizeof(ScanSmemFull);
+    cudaError_t e = cudaFuncSetAttribute(scan_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     return (int)e;
 }
 
-template <int NW> static int launch_scan_t(const ScanParams *p, const DeviceTables *d_tables, int n_sm, cudaStream_t stream) {
+extern "C" int b200_launch_scan(const ScanParams *p, const DeviceTables *d_tables, int n_sm, void *stream_) {
     // One persistent CTA per SM.  A run with fewer tiles than the chip has warps is spread out: as many CTAs as there are tiles (at
     // most one per SM) and only as many warps of each as it takes - a lone warp on an SM runs several times faster than one of 28.
+    if (!p->n_tiles) return 0;
+    const cudaStream_t stream = (cudaStream_t)stream_;
     ScanParams q = *p;
     uint32_t grid = (uint32_t)n_sm;
-    q.warps_per_cta = NW; q.static_tiles = 0;
+    q.warps_per_cta = SC_WARPS; q.static_tiles = 0;
     const uint32_t sub = p->sub_chunks;
     q.sub_chunks = 0;
-    if (q.n_tiles < grid * NW) {
+    if (q.n_tiles < grid * SC_WARPS) {
         if (grid > q.n_tiles) grid = q.n_tiles;
         q.warps_per_cta = (q.n_tiles + grid - 1) / grid;
         q.static_tiles = (grid == q.n_tiles) ? 1u : 0u;      // then warps_per_cta is 1: CTA b takes tile b ...
         if (q.static_tiles && (sub == 1 || sub == 2)) { q.sub_chunks = sub; q.warps_per_cta = TILE_CHUNKS / sub; }   // ... or its first warps share it (finish_shared_tile)
     }
-    const size_t smem = sizeof(ScanSmemFull<NW>);
-    if (q.sub_chunks) { if (q.mag_copy) scan_kernel<NW, true, true><<<grid, NW * 32, smem, stream>>>(q, d_tables); else scan_kernel<NW, true, false><<<grid, NW * 32, smem, stream>>>(q, d_tables); }
-    else { if (q.mag_copy) scan_kernel<NW, false, true><<<grid, NW * 32, smem, stream>>>(q, d_tables); else scan_kernel<NW, false, false><<<grid, NW * 32, smem, stream>>>(q, d_tables); }
+    const size_t smem = sizeof(ScanSmemFull);
+    if (q.sub_chunks) { if (q.mag_copy) scan_kernel<true, true><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); else scan_kernel<true, false><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); }
+    else { if (q.mag_copy) scan_kernel<false, true><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); else scan_kernel<false, false><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); }
     return (int)cudaGetLastError();
-}
-
-extern "C" int b200_launch_scan(const ScanParams *p, const DeviceTables *d_tables, int n_sm, void *stream) {
-    if (!p->n_tiles) return 0;
-    return launch_scan_t<SC_WARPS>(p, d_tables, n_sm, (cudaStream_t)stream);
 }

@@ -28,7 +28,7 @@ def lib():
     global _LIB
     if _LIB is None:
         import os
-        path = Path(os.environ.get("B200_DEMOD_LIB") or LIB_PATH)     # an experimental build variant of the same library (build.py)
+        path = Path(os.environ.get("B200_DEMOD_LIB") or LIB_PATH)     # another build of the same C ABI (the test suite's emulated kernels)
         if not path.exists():
             raise DemodError(f"{path} is missing: run `python -m readsb_b200.build` (nvcc, sm_90a). "
                              "There is no CPU fallback for the demodulator.")

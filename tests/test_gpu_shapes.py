@@ -1,6 +1,6 @@
 """The launch shapes where the kernels change their schedule, every receiver against an oracle of its own:
 
-- the scan kernel's three regimes (launch_scan_t, scan_kernel.cu): one CTA per tile (static tiles, a tile optionally shared by two
+- the scan kernel's three regimes (b200_launch_scan, scan_kernel.cu): one CTA per tile (static tiles, a tile optionally shared by two
   or four warps), a spread grid with dynamic claims, and the persistent grid; at the chip's own SM count and on small forced grids;
 - stage B's work units (resolve_stream): whole buffers, or sub-ranges of whole tiles of each buffer;
 - stage B CTAs in several waves (more receivers than the chip holds at two CTAs per SM), with grown filter tables at receiver 0
@@ -46,7 +46,7 @@ SC_WARPS = _sc_warps()
 
 
 def _regime(n_tiles: int, grid: int) -> str:
-    """launch_scan_t's rule (test_regime_rule_is_the_launchers pins it to the source)."""
+    """b200_launch_scan's rule (test_regime_rule_is_the_launchers pins it to the source)."""
     if n_tiles >= grid * SC_WARPS:
         return "persistent"
     return "static" if n_tiles <= grid else "spread"
@@ -495,13 +495,13 @@ def test_regime_rule_is_the_launchers():
     """The tests above choose their tile counts from _regime and their sub-ranges from _nsplit: both must be the kernels' rules, so
     that a change of a rule fails here instead of moving the tests off the boundaries they are named for."""
     src = SCAN_SRC.read_text()
-    body = re.search(r"template <int NW> static int launch_scan_t\(.*?\n\}", src, re.S).group(0)
+    body = re.search(r'extern "C" int b200_launch_scan\(.*?\n\}', src, re.S).group(0)
     assert "uint32_t grid = (uint32_t)n_sm;" in body
-    assert "if (q.n_tiles < grid * NW) {" in body
+    assert "if (q.n_tiles < grid * SC_WARPS) {" in body
     assert "if (grid > q.n_tiles) grid = q.n_tiles;" in body
     assert "q.static_tiles = (grid == q.n_tiles) ? 1u : 0u;" in body
     assert "q.warps_per_cta = TILE_CHUNKS / sub;" in body
-    assert "launch_scan_t<SC_WARPS>(" in src and SC_WARPS == 28
+    assert "q.warps_per_cta = SC_WARPS;" in body and "<<<grid, SC_WARPS * 32, smem, stream>>>" in body and SC_WARPS == 28
     assert [_regime(t, 132) for t in (131, 132, 133, 3695, 3696, 3697)] == ["static", "static", "spread", "spread", "persistent", "persistent"]
     res = RESOLVE_SRC.read_text()
     assert "const uint32_t nsplit = seg.n_bufs >= RS_WARPS ? 1u : max(1u, min((uint32_t)RS_WARPS / max(seg.n_bufs, 1u), " \
