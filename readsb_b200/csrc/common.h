@@ -149,11 +149,8 @@ struct ScanParams {
     // descriptor upload in front of the kernels.  one_seg_valid: segs / tile_seg are not read, every tile belongs to one_seg.
     Segment one_seg;
     uint32_t one_seg_valid;
-    uint32_t static_tiles;       // set by the launcher: as many CTAs as tiles, CTA b takes tile b (no claim counter)
     uint32_t warps_per_cta;      // set by the launcher: warps of each CTA that take work (a small run is spread over many SMs, few warps each)
     uint32_t need_lut;           // some segment holds uc8 IQ: the magnitude table has to be staged (a pure magnitude hand-off skips it)
-    uint32_t sub_chunks;         // caller: chunks of 512 positions per warp it asks for when the run is small (0: whole tiles); the launcher
-                                 // keeps it only with static_tiles: the TILE_CHUNKS / sub_chunks first warps of CTA b share tile b
     uint32_t long_set, short_set; // valid DF bitsets (demod_2400.c:98-128)
     int32_t nfix, fixdf;
     // per-warp private areas in global memory

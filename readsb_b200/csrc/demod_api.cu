@@ -123,7 +123,6 @@ struct b200_demod_ctx {
     bool part_fixed = false, part_off = false;     // B200_SCAN_SMS given: no tuning; B200_SCAN_PART=0: always the whole chip
     PartCal cal;
     int cal_restarts = 0;
-    int scan_sub = 1;                 // chunks per warp when a run is small enough for one CTA per tile (scan_kernel.cu, finish_shared_tile); B200_SCAN_SUB: 0 = whole tiles
     int n_sm_scan_async = 0;          // ... in pipelined runs, unless the session's measurement chose fewer (part_n, tune_partition) or B200_SCAN_SMS fixed it
     cudaStream_t stream = nullptr, own_stream = nullptr, res_stream = nullptr, copy_stream = nullptr, in_stream = nullptr;
     std::string err;
@@ -377,7 +376,6 @@ API int b200_demod_create(const b200_demod_config *cfg, b200_demod_ctx **out) {
         if (v >= 1 && v <= c->n_sm) { c->n_sm_scan = c->n_sm_scan_async = v; c->part_fixed = true; }
     }
     if (const char *e = getenv("B200_SCAN_PART")) { c->part_off = atoi(e) == 0; c->part_debug = atoi(e) == 2; }
-    if (const char *e = getenv("B200_SCAN_SUB")) { const int v = atoi(e); if (v >= 0 && v <= 2) c->scan_sub = v; }     // experiment knob (tools/gpu_latency.py)
     {   // With several steps in flight the scan kernels of later steps are already queued when a scan ends; stage B of the step
         // that just finished scanning must not wait behind them (its results gate the host), so its stream has the higher
         // priority: the block scheduler places stage B's CTAs first, the next scan's persistent CTAs follow as SMs drain, and
@@ -616,7 +614,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     ScanParams sp;
     sp.segs = sl.d_segs; sp.tile_seg = sl.d_tile_seg; sp.n_tiles = sl.ntile; sp.pos_pool = sl.d_pos_pool; sp.rec_pool = sl.d_rec_pool;
     sp.key_pool = sl.d_key_pool; sp.tile_out = sl.d_tile_out; sp.buf_acc = sl.d_buf_acc; sp.ctl = sl.d_ctl;
-    sp.rec_cap = sl.rec_cap; sp.warps_per_cta = 0; sp.static_tiles = 0; sp.need_lut = 0; sp.sub_chunks = (uint32_t)c->scan_sub;
+    sp.rec_cap = sl.rec_cap; sp.warps_per_cta = 0; sp.need_lut = 0;
     sp.one_seg_valid = one_seg ? 1u : 0u;
     if (sl.nseg) sp.one_seg = sl.h_segs[0]; else memset(&sp.one_seg, 0, sizeof sp.one_seg);
     for (uint32_t i = 0; i < sl.nseg; i++) if (!(sl.h_segs[i].flags & SEG_MAG)) sp.need_lut = 1;

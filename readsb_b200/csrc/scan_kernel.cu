@@ -27,17 +27,6 @@
 #include "common.h"
 #include "device_utils.cuh"
 
-// Trip counters for the instruction model of tools/scan_model.py: compiled in only with -DB200_SCAN_COUNTERS, which
-// only an analysis build of the test infrastructure passes; nothing of this is in the sm_90a library (its SASS is unchanged).
-#ifdef B200_SCAN_COUNTERS
-extern "C" { __attribute__((visibility("default"))) unsigned long long b200_scan_counters[16]; }
-#define SCAN_COUNT(id, n) do { if ((threadIdx.x & 31) == 0) b200_scan_counters[id] += (n); } while (0)
-#else
-#define SCAN_COUNT(id, n) do { } while (0)
-#endif
-enum { SCN_RUNS, SCN_LOOP_ITERS, SCN_WINDOW_CHUNKS, SCN_FAST_CONVERTS, SCN_EDGE_CONVERTS, SCN_Q1_ENTRIES, SCN_Q1_LOOP_TRIPS, SCN_THR_BATCHES,
-       SCN_PASS_BATCHES, SCN_PASSERS, SCN_GATE_TRIPS, SCN_SURVIVORS, SCN_SLICE_ROUNDS, SCN_SLICE_BYTES };
-
 #define SC_WARPS 28
 #define SC_MAXNREG 72                         // SC_WARPS x 32 x SC_MAXNREG <= 65536 registers per SM (other splits were slower: DESIGN.md §4, "Tried and NOT in the code")
 #define CHUNK 512
@@ -463,10 +452,6 @@ __device__ __forceinline__ void slice_round(const ScanSmem &S, WarpSmem &W, cons
     PosEntry *run_pos = P.pos_pool + (size_t)W.ctx.tile0 * SCAN_TILE;
     uint32_t rw[8];
     uint32_t kind = 0;
-    SCAN_COUNT(SCN_SLICE_ROUNDS, 1);
-#ifdef B200_SCAN_COUNTERS
-    { const bool lg = lane < cnt && ((W.surv[lane] >> 17) & 1u); const uint32_t nby = __any_sync(FULLMASK, lg) ? 14 : 7; SCAN_COUNT(SCN_SLICE_BYTES, nby); }
-#endif
     if (lane < cnt) {
         const uint32_t e = W.surv[lane];
         const uint32_t p = e & 0x3fffu, ph = (e >> 14) & 7u;
@@ -511,7 +496,6 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
         const bool have_batch = b0 < n_q1;
         uint32_t pl = 0, tried = 0, bal = 0;
         if (have_batch) {
-            SCAN_COUNT(SCN_THR_BATCHES, 1);
             const uint32_t e = b0 + lane;
             if (e < n_q1) {
                 pl = e < Q1_SMEM ? W.q1[e] : W_Q1_OVER(W, P)[e - Q1_SMEM];      // chunk-local position
@@ -523,7 +507,6 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
         if (n_pass && (!have_batch || n_pass + n_b > 32)) {      // ---- DF gates of the waiting passers
             __syncwarp();
             for (uint32_t i0 = 0; i0 < 5 * n_pass; i0 += 32) {          // five lanes per passer, one per phase
-                SCAN_COUNT(SCN_GATE_TRIPS, 1);
                 const uint32_t i_ = i0 + lane, r = i_ / 5, gph = i_ - 5 * r;
                 uint32_t g = 0, pe = 0;
                 if (r < n_pass) {
@@ -533,7 +516,6 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
                 const uint32_t bal2 = __ballot_sync(FULLMASK, g & 1u);
                 if (g & 1u) W.surv[n_surv + __popc(bal2 & lt)] = (chunk_p0 + (pe & 0xffffu)) | (gph << 14) | ((g >> 1) << 17) | ((pos_base + r) << 18);
                 n_surv += __popc(bal2);
-                SCAN_COUNT(SCN_SURVIVORS, __popc(bal2));
                 __syncwarp();
                 if (n_surv >= 32) {
                     slice_round(S, W, P, 32, lane, n_stage);
@@ -549,7 +531,6 @@ template <bool SUB> __device__ __forceinline__ void process_candidates(const Sca
         }
         if (!have_batch) break;
         if (bal) {
-            SCAN_COUNT(SCN_PASS_BATCHES, 1); SCAN_COUNT(SCN_PASSERS, n_b);
             if (tried) {
                 const uint32_t r = n_pass + __popc(bal & lt);
                 W.pass[r] = pl | (tried << 16);
@@ -577,7 +558,7 @@ __device__ __noinline__ void finish_shared_tile(WarpSmem &W0, WarpSmem &W, const
     static_assert(RUN_MAX >= TILE_CHUNKS + 3, "exchange area of finish_shared_tile");
     struct Exchange { uint32_t *sub_pos, *sub_rec; uint32_t &sub_rec_off, &sub_ok; } S = {&W0.n_pos[1], &W0.n_rec[1], W0.n_pos[TILE_CHUNKS + 1], W0.n_pos[TILE_CHUNKS + 2]};
     const RunCtx &T = W.ctx;
-    const uint32_t n_warps = TILE_CHUNKS / P.sub_chunks, tile = T.tile0;
+    const uint32_t n_warps = TILE_CHUNKS, tile = T.tile0;
     PosEntry *tile_pos = P.pos_pool + (size_t)tile * SCAN_TILE;
     const uint32_t my_pos = W.n_pos[0] - T.sub_off;
     if (lane == 0) { S.sub_pos[wid] = my_pos; S.sub_rec[wid] = n_stage; }
@@ -628,11 +609,11 @@ __device__ __noinline__ void finish_shared_tile(WarpSmem &W0, WarpSmem &W, const
     if (wid == 0 && lane == 0) { TileOut t; t.n_pos = pos_tot; t.n_rec = ok ? rec_tot : 0; t.rec_off = off; t.n_found = rec_tot; P.tile_out[tile] = t; }
 }
 
-// SUB: the launcher's small-run form, a tile shared between the warps of its CTA (finish_shared_tile).  KEEP: a Mode A/C context, the
-// magnitudes are also written to ScanParams::mag_copy.  Both are compile-time so that the plain kernel - the one the throughput is
-// measured on - carries nothing of either (measured with them as run-time tests: 4 - 6 % slower).
+// SUB: the launcher's form for a run of at most one tile per SM, a tile shared by the warps of one CTA: CTA b takes tile b without a
+// claim, and its first TILE_CHUNKS warps take one chunk of it each (finish_shared_tile).  KEEP: a Mode A/C context, the magnitudes are
+// also written to ScanParams::mag_copy.  Both are compile-time so that the plain kernel - the one the throughput is measured on -
+// carries nothing of either (measured with them as run-time tests: 4 - 6 % slower).
 template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kernel(const __grid_constant__ ScanParams P, const DeviceTables *__restrict__ tables) {
-    const uint32_t sub_chunks = SUB ? P.sub_chunks : 0u;
     constexpr uint32_t SC_THREADS = SC_WARPS * 32;
     extern __shared__ uint4 smem_raw[];
     ScanSmemFull &F = *reinterpret_cast<ScanSmemFull *>(smem_raw);
@@ -663,14 +644,11 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
     __syncwarp();
 
     uint32_t pend_tile = 0, pend_n = 0;       // tiles already claimed but not processed yet (a claim that crossed a segment boundary)
-    bool static_done = false;
     for (;;) {
         // ---- claim a run: guided self-scheduling, then cut at the segment boundary --------------------------------------
         if (!pend_n) {
             uint32_t start = 0, n = 0;
-            if (P.static_tiles) {                 // one tile per CTA (a run of a few dozen tiles): no claim, no atomic round trip
-                if (static_done) break;
-                static_done = true;
+            if (SUB) {                            // one tile per CTA (a run of a few dozen tiles): no claim, no atomic round trip
                 start = blockIdx.x; n = 1;
             } else if (lane == 0) {
                 const uint32_t cur = *reinterpret_cast<volatile uint32_t *>(&P.ctl->tile_counter);
@@ -681,7 +659,7 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
                     if (start >= P.n_tiles) n = 0; else n = min(n, P.n_tiles - start);
                 }
             }
-            if (!P.static_tiles) { start = __shfl_sync(FULLMASK, start, 0); n = __shfl_sync(FULLMASK, n, 0); }
+            if (!SUB) { start = __shfl_sync(FULLMASK, start, 0); n = __shfl_sync(FULLMASK, n, 0); }
             pend_tile = start; pend_n = n;
             if (!pend_n) break;
         }
@@ -697,9 +675,8 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
             const Segment &seg = *reinterpret_cast<const Segment *>(W.seg);
             const uint32_t tile0 = pend_tile, n_tiles_run = min(pend_n, seg.tile_begin + seg.n_tiles - tile0);
             pend_tile += n_tiles_run; pend_n -= n_tiles_run;
-            n_chunks = n_tiles_run * TILE_CHUNKS;
-            const uint32_t sub_off = SUB ? wid * sub_chunks * CHUNK : 0u;             // a tile shared between warps: this warp's chunks of it
-            if (SUB) n_chunks = sub_chunks;
+            n_chunks = SUB ? 1u : n_tiles_run * TILE_CHUNKS;
+            const uint32_t sub_off = SUB ? wid * CHUNK : 0u;                         // a tile shared between warps: this warp's chunk of it
             if (lane == 0) {
                 const uint32_t x0 = (tile0 - seg.tile_begin) * SCAN_TILE + sub_off;   // run origin in tile coordinates (x = data index + lead)
                 T.x0 = x0; T.tile0 = tile0; T.n_tiles = n_tiles_run; T.n_chunks = n_chunks; T.tile_rel0 = tile0 - seg.tile_begin; T.sub_off = sub_off;
@@ -721,7 +698,6 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
         __syncwarp();
 
         uint32_t n_q1 = 0, n_surv = 0, n_stage = 0;
-        SCAN_COUNT(SCN_RUNS, 1);
         uint32_t ms = 0;          // ring slot of chunk k's magnitudes; ticks of chunk k sit in slot k & 1
         // Chunks in the interior of the data and of a reference buffer need no case analysis: `fast_left` counts how many chunks
         // after the one just classified are of the same kind (staged, converted by the fast path, counted for buffer `fast_buf`);
@@ -732,9 +708,7 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
 #pragma unroll 1
         for (int k = -2; k <= (int)n_chunks; k++) {
             uint32_t mask = 0;
-            SCAN_COUNT(SCN_LOOP_ITERS, 1);
             if (k >= 0) {
-                SCAN_COUNT(SCN_WINDOW_CHUNKS, 1);
                 // ---- window(k): pre-check + tick map -----------------------------------------------------------------
                 mask = window_pass(W, ms * CHUNK + lane * 16, (k & 1) * TICK_CW, lane, (k & 1) == 0, W_TICKG(W, P) + k * TICK_CW);
                 if ((uint32_t)k < k_int_lo || (uint32_t)k >= k_int_hi) {      // positions outside [p_lo, p_hi) are not preamble starts
@@ -786,7 +760,6 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
             // ---- convert(k+2) into the slot chunk k-1 occupied ------------------------------------------------------
             if (more) {
                 const uint32_t msn = k < 0 ? cn : (ms == 0 ? 2 : ms - 1);       // (ms + 2) % 3; the first two chunks fill slots 0 and 1
-                SCAN_COUNT(fast ? SCN_FAST_CONVERTS : SCN_EDGE_CONVERTS, 1);
                 if (fast) convert_chunk_fast<KEEP>(S, W, P, T.is_mag, msn, lane, count_buf, cn);
                 else {
                     if (all_data) stage_wait();      // staged, but this chunk straddles a buffer boundary: the edge path loads it itself
@@ -798,9 +771,6 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
                 uint32_t off = warp_excl_scan(__popc(mask), lane, &n_q1);
                 const uint32_t i0 = lane * 16;                   // chunk-local
                 uint32_t mb = mask;
-#ifdef B200_SCAN_COUNTERS
-                { const uint32_t trips = __reduce_max_sync(FULLMASK, (uint32_t)__popc(mask)); SCAN_COUNT(SCN_Q1_LOOP_TRIPS, trips); SCAN_COUNT(SCN_Q1_ENTRIES, n_q1); }
-#endif
                 while (mb) {
                     const uint32_t b = __ffs(mb) - 1; mb &= mb - 1;
                     if (off < Q1_SMEM) W.q1[off] = (uint16_t)(i0 + b); else W_Q1_OVER(W, P)[off - Q1_SMEM] = (uint16_t)(i0 + b);
@@ -864,17 +834,15 @@ extern "C" int b200_launch_scan(const ScanParams *p, const DeviceTables *d_table
     const cudaStream_t stream = (cudaStream_t)stream_;
     ScanParams q = *p;
     uint32_t grid = (uint32_t)n_sm;
-    q.warps_per_cta = SC_WARPS; q.static_tiles = 0;
-    const uint32_t sub = p->sub_chunks;
-    q.sub_chunks = 0;
+    q.warps_per_cta = SC_WARPS;
     if (q.n_tiles < grid * SC_WARPS) {
         if (grid > q.n_tiles) grid = q.n_tiles;
         q.warps_per_cta = (q.n_tiles + grid - 1) / grid;
-        q.static_tiles = (grid == q.n_tiles) ? 1u : 0u;      // then warps_per_cta is 1: CTA b takes tile b ...
-        if (q.static_tiles && (sub == 1 || sub == 2)) { q.sub_chunks = sub; q.warps_per_cta = TILE_CHUNKS / sub; }   // ... or its first warps share it (finish_shared_tile)
     }
+    const bool shared = grid == q.n_tiles;            // as many CTAs as tiles: CTA b takes tile b, one chunk per warp (finish_shared_tile)
+    if (shared) q.warps_per_cta = TILE_CHUNKS;
     const size_t smem = sizeof(ScanSmemFull);
-    if (q.sub_chunks) { if (q.mag_copy) scan_kernel<true, true><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); else scan_kernel<true, false><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); }
+    if (shared) { if (q.mag_copy) scan_kernel<true, true><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); else scan_kernel<true, false><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); }
     else { if (q.mag_copy) scan_kernel<false, true><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); else scan_kernel<false, false><<<grid, SC_WARPS * 32, smem, stream>>>(q, d_tables); }
     return (int)cudaGetLastError();
 }

@@ -156,17 +156,16 @@ def sanitizer_runtime(sanitize: str) -> str:
     return subprocess.run([cxx, f"-print-file-name={name}"], capture_output=True, text=True, check=True).stdout.strip()
 
 
-def build(force: bool = False, verbose: bool = False, sanitize: str | None = None, defines: tuple = ()) -> Path:
+def build(force: bool = False, verbose: bool = False, sanitize: str | None = None) -> Path:
     """sanitize = "address": heap "device" buffers get redzones, so a kernel reading or writing past a pool, an arena or a
     result array is reported with the source line; "undefined": oversized shifts, signed overflow, misaligned vector loads —
     the places where C++ on the CPU and the GPU's semantics could differ."""
     srcs = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h"))
     deps = srcs + [HERE / "cuda_runtime.h", HERE / "emu_rt.cpp", Path(__file__), ROOT / "include" / "b200_demod.h"]
-    tag = "_".join(([sanitize] if sanitize else []) + [d.lower() for d in defines])
-    LIB = BUILD / ("libb200demod_emu.so" if not tag else f"libb200demod_emu_{tag}.so")
+    LIB = BUILD / ("libb200demod_emu.so" if not sanitize else f"libb200demod_emu_{sanitize}.so")
     if not force and LIB.exists() and all(d.stat().st_mtime <= LIB.stat().st_mtime for d in deps):
         return LIB
-    gen = BUILD / ("src" if not tag else f"src_{tag}")
+    gen = BUILD / ("src" if not sanitize else f"src_{sanitize}")
     if gen.exists():
         shutil.rmtree(gen)
     gen.mkdir(parents=True)
@@ -181,7 +180,7 @@ def build(force: bool = False, verbose: bool = False, sanitize: str | None = Non
     # -ffp-contract=off mirrors nvcc --fmad=false; -O1 keeps frames small and the build quick; -fno-strict-aliasing because the
     # kernels reinterpret shared memory freely (nvcc does not do type-based alias analysis on it either)
     san = [f"-fsanitize={sanitize}", "-fno-omit-frame-pointer"] if sanitize else []
-    cmd = [cxx, "-std=c++17", "-O1", "-g", "-fPIC", "-shared", *san, *[f"-D{d}" for d in defines], "-ffp-contract=off", "-fno-strict-aliasing", "-fvisibility=hidden",
+    cmd = [cxx, "-std=c++17", "-O1", "-g", "-fPIC", "-shared", *san, "-ffp-contract=off", "-fno-strict-aliasing", "-fvisibility=hidden",
            "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-Wno-unused-variable", "-Wno-unused-but-set-variable",
            "-include", str(HERE / "cuda_runtime.h"), "-I", str(HERE), "-I", str(gen), "-I", str(ROOT / "include"),
            *map(str, cpp), str(HERE / "emu_rt.cpp"), "-o", str(LIB), "-lpthread"]

@@ -1,7 +1,7 @@
 """The launch shapes where the kernels change their schedule, every receiver against an oracle of its own:
 
-- the scan kernel's three regimes (b200_launch_scan, scan_kernel.cu): one CTA per tile (static tiles, a tile optionally shared by two
-  or four warps), a spread grid with dynamic claims, and the persistent grid; at the chip's own SM count and on small forced grids;
+- the scan kernel's three regimes (b200_launch_scan, scan_kernel.cu): one CTA per tile (static tiles, each shared by four warps), a
+  spread grid with dynamic claims, and the persistent grid; at the chip's own SM count and on small forced grids;
 - stage B's work units (resolve_stream): whole buffers, or sub-ranges of whole tiles of each buffer;
 - stage B CTAs in several waves (more receivers than the chip holds at two CTAs per SM), with grown filter tables at receiver 0
   and past the first 256 receivers;
@@ -147,7 +147,6 @@ def _check_regime(path, where, grid, fmt=FORMAT_UC8, mode_ac=False, seed=1):
 def test_scan_regimes_at_the_chips_sm_count(cuda, monkeypatch, path, where):
     """Tile counts one below, at and one above each regime boundary of a grid of the chip's SMs, blocking and three steps in flight."""
     monkeypatch.delenv("B200_SCAN_SMS", raising=False)
-    monkeypatch.delenv("B200_SCAN_SUB", raising=False)
     monkeypatch.setenv("B200_SCAN_PART", "0")      # pipelined steps keep the whole chip (no measured partition moving the boundary)
     _check_regime(path, where, _sms(), seed=3 + WHERES.index(where))
 
@@ -157,7 +156,6 @@ def test_scan_regimes_at_the_chips_sm_count(cuda, monkeypatch, path, where):
 def test_scan_regimes_with_modeac_and_sc16(cuda, monkeypatch, kind, where):
     """The scan kernel that keeps its magnitudes for Mode A/C, and sc16 input (magnitude segments over the converter's slab)."""
     monkeypatch.delenv("B200_SCAN_SMS", raising=False)
-    monkeypatch.delenv("B200_SCAN_SUB", raising=False)
     monkeypatch.setenv("B200_SCAN_PART", "0")
     _check_regime("device_async", where, _sms(), fmt=FORMAT_SC16 if kind == "sc16" else FORMAT_UC8, mode_ac=kind == "modeac", seed=20)
 
@@ -168,7 +166,6 @@ def test_scan_regimes_with_modeac_and_sc16(cuda, monkeypatch, kind, where):
 def test_scan_regimes_on_forced_small_grids(cuda, monkeypatch, grid):
     assert grid <= _sms()
     monkeypatch.setenv("B200_SCAN_SMS", str(grid))          # read by create: the scan grid of blocking and pipelined runs
-    monkeypatch.delenv("B200_SCAN_SUB", raising=False)
     for i, where in enumerate(WHERES):
         if _target(where, grid)[0] == 0:
             continue
@@ -178,13 +175,11 @@ def test_scan_regimes_on_forced_small_grids(cuda, monkeypatch, grid):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("grid", [3, 7])
-@pytest.mark.parametrize("sub", [0, 1, 2])
-def test_tiles_shared_between_warps(cuda, monkeypatch, grid, sub):
-    """n_tiles == grid: CTA b takes tile b whole (B200_SCAN_SUB=0), or its first four (1) or two (2) warps share it."""
+def test_tiles_shared_between_warps(cuda, monkeypatch, grid):
+    """n_tiles == grid: CTA b takes tile b, and its first four warps share it, one chunk each."""
     monkeypatch.setenv("B200_SCAN_SMS", str(grid))
-    monkeypatch.setenv("B200_SCAN_SUB", str(sub))
     for path in ("device", "device_async"):
-        _check_regime(path, "grid", grid, seed=40 + sub)
+        _check_regime(path, "grid", grid, seed=41)
 
 
 @pytest.mark.gpu
@@ -192,7 +187,6 @@ def test_tiles_shared_between_warps(cuda, monkeypatch, grid, sub):
 def test_claims_cross_many_short_segments(cuda, monkeypatch, grid):
     """Receivers of 1, 2, 3, 5 and 9 tiles in one run: claims of up to 8 tiles cut through several segments, quads end partway."""
     monkeypatch.setenv("B200_SCAN_SMS", str(grid))
-    monkeypatch.delenv("B200_SCAN_SUB", raising=False)
     counts = [1, 2, 3, 5, 9] * 12
     T = sum(counts)
     assert _regime(T, grid) == "persistent" and min(-(-T // (grid * SC_WARPS)), 8) >= 3      # the first claims take 8 or 3 tiles
@@ -499,8 +493,9 @@ def test_regime_rule_is_the_launchers():
     assert "uint32_t grid = (uint32_t)n_sm;" in body
     assert "if (q.n_tiles < grid * SC_WARPS) {" in body
     assert "if (grid > q.n_tiles) grid = q.n_tiles;" in body
-    assert "q.static_tiles = (grid == q.n_tiles) ? 1u : 0u;" in body
-    assert "q.warps_per_cta = TILE_CHUNKS / sub;" in body
+    assert "q.warps_per_cta = (q.n_tiles + grid - 1) / grid;" in body
+    assert "const bool shared = grid == q.n_tiles;" in body
+    assert "if (shared) q.warps_per_cta = TILE_CHUNKS;" in body and "if (shared) { if (q.mag_copy) scan_kernel<true, true><<<" in body
     assert "q.warps_per_cta = SC_WARPS;" in body and "<<<grid, SC_WARPS * 32, smem, stream>>>" in body and SC_WARPS == 28
     assert [_regime(t, 132) for t in (131, 132, 133, 3695, 3696, 3697)] == ["static", "static", "spread", "spread", "persistent", "persistent"]
     res = RESOLVE_SRC.read_text()
