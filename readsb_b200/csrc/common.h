@@ -1,4 +1,4 @@
-// common.h — structures shared by the kernels (demod_kernels.cu) and the C ABI (demod_api.cu).
+// common.h — structures shared by the kernels (*_kernel.cu) and the C ABI (demod_api.cu).
 //
 // Data layout in HBM (see DESIGN.md):
 //   * input: 2 bytes per sample either way (uc8 I,Q pair, or one uint16 magnitude), so one
@@ -119,12 +119,10 @@ struct StreamState {
 struct RunCtl {
     uint32_t rec_alloc;      // atomic bump pointer into rec_pool
     uint32_t pad0_;
-    uint32_t overflow;       // bit0: rec_pool exhausted, bit1: per-tile queue capacity exceeded, bit2: frame capacity,
-                             // bit3: a receiver's ICAO tables have to grow before this run (StreamState.grow_log2), bit4: stage B skipped
-                             // because the step ahead has to be repeated, bit5: Mode A/C candidate / output capacity exceeded
+    uint32_t overflow;       // OV_* bits
     uint32_t tile_counter;   // dynamic tile scheduler
     uint32_t total_frames;
-    uint32_t stage_need;     // with overflow bit1: the largest number of live records one tile produced (staging areas too small)
+    uint32_t stage_need;     // with OV_STAGING_FULL: the largest number of live records one tile produced (staging areas too small)
     uint32_t pad_[2];
     uint32_t cap_check;      // stage B's capacity check of this run (resolve_kernel): 0 not yet, 1 in progress, CAP_GO / CAP_STOP made
     uint32_t pad1_[3];
@@ -132,7 +130,15 @@ struct RunCtl {
 #define CAP_STOP 2u          // cap_check: made, stage B must not run (this step is going to be repeated)
 #define CAP_GO   3u          // cap_check: made, stage B runs
 
-#define RUN_REPEAT_BITS (1u | 2u | 8u | 16u)   // stage B did not run (or must not): the host repairs and repeats the step
+// RunCtl.overflow
+#define OV_REC_POOL_FULL 0x01u   // stage A: rec_pool exhausted
+#define OV_STAGING_FULL  0x02u   // stage A: a run of tiles has more live records than the per-warp staging areas hold (RunCtl.stage_need)
+#define OV_FRAME_CAP     0x04u   // stage B: a receiver's frame slots exceeded
+#define OV_FILTER_GROW   0x08u   // a receiver's ICAO tables have to grow before this run (StreamState.grow_log2)
+#define OV_SKIPPED       0x10u   // stage B skipped because the step ahead has to be repeated
+#define OV_MODEAC_CAP    0x20u   // Mode A/C candidate / output capacity exceeded
+#define OV_STAGE_A_FAILED (OV_REC_POOL_FULL | OV_STAGING_FULL)   // stage A's output is incomplete
+#define RUN_REPEAT_BITS (OV_STAGE_A_FAILED | OV_FILTER_GROW | OV_SKIPPED)   // stage B did not run (or must not): the host repairs and repeats the step
 
 struct ScanParams {
     const Segment *segs;
@@ -166,22 +172,6 @@ struct ScanParams {
     uint16_t *mag_copy;
 };
 
-struct FinalizeParams {
-    const Segment *segs;
-    const uint32_t *stream_seg_begin;
-    uint32_t n_streams;
-    b200_frame *frames;
-    uint32_t *frame_span;             // [n_streams][2]: where the receiver's frames start in `packed`, and how many there are
-    Segment one_seg;                  // (see ScanParams) the run's only segment, when one_seg_valid
-    uint32_t one_seg_valid;
-    uint32_t frame_cap;
-    b200_frame *packed;               // all frames of the run: each receiver's in order, in one contiguous range (frame_span)
-    const Rec *rec_pool;
-    BufAcc *buf_acc;
-    StreamState *state;
-    const uint16_t *lut_full;         // 65536-entry UC8 table in global memory
-};
-
 struct ResolveParams {
     const Segment *segs;
     const uint32_t *stream_seg_begin; // per stream: first segment index (segments sorted by stream); [n_streams+1]
@@ -204,7 +194,9 @@ struct ResolveParams {
     Segment one_seg;                  // (see ScanParams) the run's only segment, when one_seg_valid
     uint32_t one_seg_valid;
     uint32_t solo;                    // one receiver in the context: resolve_solo_kernel (see resolve_kernel.cu)
-    FinalizeParams fin;               // what the finalizer needs
+    uint32_t *frame_span;             // [n_streams][2]: where the receiver's frames start in `packed`, and how many there are
+    b200_frame *packed;               // all frames of the run: each receiver's in order, in one contiguous range (frame_span)
+    const uint16_t *lut_full;         // 65536-entry UC8 table in global memory (the finalizer's signal power)
     // (solo, optional) the kernel PUBLISHES the run's result block itself: copies publish_head bytes + the packed frames from
     // publish_src (device) to publish_dst (the host's pinned copy, mapped into the device's address space) - no device-to-host
     // copy operation in the stream - and then zeroes the control block and the per-buffer sums for the next run (no memset either)
@@ -277,7 +269,7 @@ struct Sc16Params {
 struct BeastParams {                 // beast_kernel.cu
     const Segment *segs;
     const uint32_t *stream_seg_begin;
-    const b200_frame *frames;         // packed (FinalizeParams::packed)
+    const b200_frame *frames;         // packed (ResolveParams::packed)
     const uint32_t *frame_span;       // [stream][2]: first frame, frame count
     const b200_buffer_result *buf_out;
     const b200_modeac *ac;            // packed in buffer order, or null
@@ -302,7 +294,7 @@ struct DeviceTables {
 #ifdef __cplusplus
 extern "C" {
 #endif
-// kernel launch wrappers implemented in demod_kernels.cu (stream is a cudaStream_t)
+// kernel launch wrappers implemented in the *_kernel.cu files (stream is a cudaStream_t)
 int b200_scan_warps(int n_sm);      // warps of the (persistent) scan kernel's grid
 int b200_scan_tick_words(void);     // words of tick scratch per warp
 int b200_launch_scan(const ScanParams *p, const DeviceTables *d_tables, int n_sm, void *stream);
@@ -316,8 +308,7 @@ int b200_launch_modeac(const AcScanParams *sp, const AcWalkParams *wp, int n_sm,
 int b200_prepare_convert(void);
 int b200_launch_sc16_convert(const Sc16Params *p, void *stream);
 int b200_launch_beast(const BeastParams *p, uint32_t n_streams, void *stream);
-int b200_launch_modeac_stats(const AcWalkParams *wp, const uint32_t *prefix, void *stream);
-int b200_launch_ac_pack(const b200_modeac *ac_out, const uint32_t *count, uint32_t *prefix, b200_modeac *packed, uint32_t n_units, uint32_t cap, RunCtl *ctl, void *stream);
+int b200_launch_modeac_pack(const AcWalkParams *wp, uint32_t n_bufs, uint32_t *prefix, b200_modeac *packed, void *stream);
 int b200_launch_icao_op(StreamState *state, uint32_t stream, int op, uint32_t addr, int *d_result, void *cstream);
 #ifdef __cplusplus
 }

@@ -68,7 +68,7 @@ struct Slot {
     BufAcc *d_buf_acc = nullptr, *h_buf_acc = nullptr;
     b200_buffer_result *d_buf_out = nullptr, *h_buf_out = nullptr;
     b200_frame *d_frames = nullptr, *d_packed = nullptr, *h_packed = nullptr;
-    uint32_t *d_frame_span = nullptr, *h_frame_span = nullptr;    // per receiver: first packed frame, frame count (FinalizeParams)
+    uint32_t *d_frame_span = nullptr, *h_frame_span = nullptr;    // per receiver: first packed frame, frame count (ResolveParams)
     uint32_t *d_addable = nullptr;    // [S] filter adds this run can make at most (scan kernel -> capacity check, which zeroes it again)
     // Mode A/C (contexts created with B200_CFG_MODE_AC)
     uint32_t *d_ac_bitmap = nullptr, *d_ac_noise = nullptr;
@@ -81,8 +81,8 @@ struct Slot {
     size_t desc_bytes = 0;            // bytes of the descriptor block this run uploads
     bool upload_tiles = true;
     std::vector<uint32_t> stream_buf_begin;   // [n_streams+1] into h_buf_out
-    cudaEvent_t ev[8] = {};                   // 0 scan begin, 1 scan end, 2 resolve end, 3 finalize end, 4 results on host,
-                                              // 5 result copies done, 6 Mode A/C scan + walk done, 7 descriptors uploaded
+    cudaEvent_t ev[7] = {};                   // 0 scan begin, 1 scan end, 2 stage B end, 3 results on host, 4 result copies done,
+                                              // 5 Mode A/C scan + walk done, 6 descriptors uploaded
     float ms[5] = {0, 0, 0, 0, 0};
     uint32_t launches = 0;
     uint32_t first_frames = 0;        // packed frames that came with the result block's copy
@@ -608,7 +608,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     if (!(publish && sl.res_clean && sl.nbuf <= sl.clean_bufs))
         CU(c, cudaMemcpyAsync(sl.d_res, c->h_zero, sizeof(RunCtl) + (size_t)sl.nbuf * sizeof(BufAcc), cudaMemcpyHostToDevice, pre));
     sl.res_clean = false; sl.published = publish; sl.timed = timing;
-    if (pre != scan) { CU(c, cudaEventRecord(sl.ev[7], pre)); CU(c, cudaStreamWaitEvent(scan, sl.ev[7], 0)); }
+    if (pre != scan) { CU(c, cudaEventRecord(sl.ev[6], pre)); CU(c, cudaStreamWaitEvent(scan, sl.ev[6], 0)); }
     sl.launches = 0;
 
     ScanParams sp;
@@ -651,14 +651,9 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
         aw.noise = sl.d_ac_noise; aw.lut_full = c->d_lut_full; aw.ac_out = sl.d_ac_out; aw.ac_count = sl.d_ac_count; aw.per_buf_cap = c->ac_cap;
         aw.state = c->d_state; aw.ctl = sl.d_ctl;
         { int r = b200_launch_modeac(&as, &aw, c->n_sm, scan); if (r) return fail(c, B200_E_CUDA, "mode a/c launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += 3; }
-        CU(c, cudaEventRecord(sl.ev[6], scan));
+        CU(c, cudaEventRecord(sl.ev[5], scan));
     }
 
-    FinalizeParams fp;
-    fp.segs = sl.d_segs; fp.stream_seg_begin = sl.d_stream_seg_begin; fp.n_streams = S; fp.frames = sl.d_frames;
-    fp.frame_span = sl.d_frame_span; fp.frame_cap = c->frame_cap; fp.packed = sl.d_packed;
-    fp.buf_acc = sl.d_buf_acc; fp.state = c->d_state; fp.lut_full = c->d_lut_full; fp.rec_pool = sl.d_rec_pool;
-    fp.one_seg = sp.one_seg; fp.one_seg_valid = sp.one_seg_valid;
     const bool solo = S == 1;          // one receiver: resolve_solo_kernel (also publishes its results / carries the halo)
     ResolveParams rp;
     rp.segs = sl.d_segs; rp.stream_seg_begin = sl.d_stream_seg_begin; rp.n_streams = S; rp.pos_pool = sl.d_pos_pool;
@@ -666,7 +661,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     rp.state = c->d_state; rp.frames = sl.d_frames; rp.frame_cap = c->frame_cap; rp.per_buf_cap = c->cfg.buf_samples / 113 + 2;
     rp.ctl = sl.d_ctl; rp.prev_stop = prev_stop; rp.stop_out = c->d_stop + (&sl - c->slot); rp.ttl_ms = c->cfg.icao_ttl_ms; rp.stream_addable = sl.d_addable;
     rp.one_seg = sp.one_seg; rp.one_seg_valid = sp.one_seg_valid;
-    rp.solo = solo ? 1u : 0u; rp.fin = fp;
+    rp.solo = solo ? 1u : 0u; rp.frame_span = sl.d_frame_span; rp.packed = sl.d_packed; rp.lut_full = c->d_lut_full;
     rp.publish_src = nullptr; rp.publish_dst = nullptr; rp.publish_head = 0; rp.publish_clear = 0;
     rp.carry_dst = nullptr; rp.carry_src = nullptr;
     if (solo && sl.carry_in_kernel != 0xffffffffu) {      // host-buffer run of one receiver: the halo carry rides in the stage B kernel
@@ -679,12 +674,11 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     }
     { const int grown = !c->icao_grown.empty();
       int r = b200_launch_resolve(&rp, grown, res); if (r) return fail(c, B200_E_CUDA, "resolve launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += solo ? 1 : 1 + grown; }
-    if (timing) { CU(c, cudaEventRecord(sl.ev[2], res)); CU(c, cudaEventRecord(sl.ev[3], res)); }     // (stage B and finalizer: one launch)
+    if (timing) CU(c, cudaEventRecord(sl.ev[2], res));
 
     if (mode_ac) {      // per-buffer reply lists -> one packed array in buffer order, receiver statistics
-        if (res != scan) CU(c, cudaStreamWaitEvent(res, sl.ev[6], 0));
-        { int r = b200_launch_ac_pack(sl.d_ac_out, sl.d_ac_count, sl.d_ac_prefix, sl.d_ac_packed, sl.nbuf, c->ac_cap, sl.d_ctl, res); if (r) return fail(c, B200_E_CUDA, "mode a/c pack launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += 2; }
-        { int r = b200_launch_modeac_stats(&aw, sl.d_ac_prefix, res); if (r) return fail(c, B200_E_CUDA, "mode a/c stats launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches++; }
+        if (res != scan) CU(c, cudaStreamWaitEvent(res, sl.ev[5], 0));
+        { int r = b200_launch_modeac_pack(&aw, sl.nbuf, sl.d_ac_prefix, sl.d_ac_packed, res); if (r) return fail(c, B200_E_CUDA, "mode a/c pack launch: %s", cudaGetErrorString((cudaError_t)r)); sl.launches += 3; }
         CU(c, cudaMemcpyAsync(sl.h_ac_prefix, sl.d_ac_prefix, ((size_t)sl.nbuf + 1) * 4, cudaMemcpyDeviceToHost, res));
     }
 
@@ -692,41 +686,47 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     sl.first_frames = (uint32_t)std::min<size_t>(FIRST_COPY_FRAMES, (size_t)S * c->frame_cap);
     if (publish) sl.first_frames = 0xffffffffu;          // the kernel has put every frame into the host's copy
     else CU(c, cudaMemcpyAsync(sl.h_res, sl.d_res, sl.res_head + (size_t)sl.first_frames * sizeof(b200_frame), cudaMemcpyDeviceToHost, res));
-    if (timing) CU(c, cudaEventRecord(sl.ev[4], res));
+    if (timing) CU(c, cudaEventRecord(sl.ev[3], res));
     return B200_OK;
 }
 
-// Second half: wait for the first result copy, fetch the frames, derive the timings.  Returns B200_OK, or a positive
-// value when the run has to be repeated: 1 = record pool too small, 2 = dense-tile scratch arena needed, 3 = skipped
-// because the step before it had to be repeated, 4 = a receiver's ICAO filter tables have to grow first.
+// Why a run has to be repeated, after the repair regrow() makes (positive: never B200_OK or an error code)
+enum Repeat : int {
+    REPEAT_REC_POOL = 1,       // record pool too small
+    REPEAT_STAGING = 2,        // per-warp record staging areas too small
+    REPEAT_SKIPPED = 3,        // stage B skipped because the step before it had to be repeated
+    REPEAT_FILTER_GROW = 4,    // a receiver's ICAO filter tables have to grow first
+};
+
+// Second half: wait for the first result copy, fetch the frames, derive the timings.  Returns B200_OK, an error, or the
+// Repeat reason when the run has to be repeated.
 static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
-    if (sl.timed) CU(c, cudaEventSynchronize(sl.ev[4])); else CU(c, cudaStreamSynchronize(res));
+    if (sl.timed) CU(c, cudaEventSynchronize(sl.ev[3])); else CU(c, cudaStreamSynchronize(res));
     if (sl.published) { sl.res_clean = true; sl.clean_bufs = sl.nbuf; }     // the kernel zeroed RunCtl + BufAcc[] after publishing them
     const uint32_t ov = sl.h_ctl->overflow;
-    if (ov & 1u) return 1;
-    if ((ov & 2u) && sl.h_ctl->stage_need > c->stage_cap) return 2;
-    if (ov & 16u) return 3;
-    if (ov & 8u) return 4;
-    if (ov & 2u) return fail(c, B200_E_OVERFLOW, "a run of tiles exceeded the record staging capacity even after regrowth");
-    if (ov & 4u) return fail(c, B200_E_OVERFLOW, "per-stream frame capacity exceeded");
-    if (ov & 32u) return fail(c, B200_E_OVERFLOW, "Mode A/C candidate capacity exceeded");
+    if (ov & OV_REC_POOL_FULL) return REPEAT_REC_POOL;
+    if ((ov & OV_STAGING_FULL) && sl.h_ctl->stage_need > c->stage_cap) return REPEAT_STAGING;
+    if (ov & OV_SKIPPED) return REPEAT_SKIPPED;
+    if (ov & OV_FILTER_GROW) return REPEAT_FILTER_GROW;
+    if (ov & OV_STAGING_FULL) return fail(c, B200_E_OVERFLOW, "a run of tiles exceeded the record staging capacity even after regrowth");
+    if (ov & OV_FRAME_CAP) return fail(c, B200_E_OVERFLOW, "per-stream frame capacity exceeded");
+    if (ov & OV_MODEAC_CAP) return fail(c, B200_E_OVERFLOW, "Mode A/C candidate capacity exceeded");
     const bool mode_ac = (c->cfg.flags & B200_CFG_MODE_AC) != 0;
     const uint32_t total_ac = mode_ac ? sl.h_ac_prefix[sl.nbuf] : 0;
     sl.ms[3] = 0;
-    if (mode_ac && sl.timed) cudaEventElapsedTime(&sl.ms[3], sl.ev[1], sl.ev[6]);       // Mode A/C noise + scan + walk kernels
+    if (mode_ac && sl.timed) cudaEventElapsedTime(&sl.ms[3], sl.ev[1], sl.ev[5]);       // Mode A/C noise + scan + walk kernels
     if (total_ac) CU(c, cudaMemcpyAsync(sl.h_ac_packed, sl.d_ac_packed, (size_t)total_ac * sizeof(b200_modeac), cudaMemcpyDeviceToHost, c->copy_stream));
     const uint32_t total = sl.h_ctl->total_frames;
     sl.run_frames = total;
-    if (total_ac && total <= sl.first_frames) { CU(c, cudaEventRecord(sl.ev[5], c->copy_stream)); CU(c, cudaEventSynchronize(sl.ev[5])); }
+    if (total_ac && total <= sl.first_frames) { CU(c, cudaEventRecord(sl.ev[4], c->copy_stream)); CU(c, cudaEventSynchronize(sl.ev[4])); }
     const bool more_frames = total > sl.first_frames;
     if (more_frames) {
         // The frame copy must not queue behind the NEXT step's stage B on the resolve stream: its own stream,
-        // ordered after this slot's finalize only (ev[4] already completed: finalize is done).
-        (void)res;
+        // ordered after this slot's stage B only (ev[3] already completed: stage B is done).
         CU(c, cudaMemcpyAsync(sl.h_packed + sl.first_frames, sl.d_packed + sl.first_frames, (size_t)(total - sl.first_frames) * sizeof(b200_frame),
                               cudaMemcpyDeviceToHost, c->copy_stream));
-        CU(c, cudaEventRecord(sl.ev[5], c->copy_stream));
-        CU(c, cudaEventSynchronize(sl.ev[5]));
+        CU(c, cudaEventRecord(sl.ev[4], c->copy_stream));
+        CU(c, cudaEventSynchronize(sl.ev[4]));
     }
     for (uint32_t b = 0; b < sl.nbuf; b++) {
         sl.h_buf_out[b].sum_level = sl.h_buf_acc[b].sum_level;
@@ -741,8 +741,8 @@ static int collect(b200_demod_ctx *c, Slot &sl, cudaStream_t res) {
     if (sl.timed) {
         cudaEventElapsedTime(&sl.ms[1], sl.ev[0], sl.ev[1]);
         cudaEventElapsedTime(&sl.ms[2], sl.ev[1], sl.ev[2]);
-        cudaEventElapsedTime(&sl.ms[0], sl.ev[0], (more_frames || total_ac) ? sl.ev[5] : sl.ev[4]);
-        cudaEventElapsedTime(&sl.ms[4], sl.ev[3], (more_frames || total_ac) ? sl.ev[5] : sl.ev[4]);
+        cudaEventElapsedTime(&sl.ms[0], sl.ev[0], (more_frames || total_ac) ? sl.ev[4] : sl.ev[3]);
+        cudaEventElapsedTime(&sl.ms[4], sl.ev[2], (more_frames || total_ac) ? sl.ev[4] : sl.ev[3]);
     } else sl.ms[0] = sl.ms[1] = sl.ms[2] = sl.ms[4] = 0;
     return B200_OK;
 }
@@ -774,9 +774,11 @@ static int grow_icao_tables(b200_demod_ctx *c) {
 }
 
 // Repairs after collect() asked for a repeat.  Every slot gets the new capacity so that later steps do not trip again.
-static int regrow(b200_demod_ctx *c, Slot &sl, int why) {
-    if (why == 4) return grow_icao_tables(c);
-    if (why == 1) {
+static int regrow(b200_demod_ctx *c, Slot &sl, Repeat why) {
+    switch (why) {
+    case REPEAT_FILTER_GROW: return grow_icao_tables(c);
+    case REPEAT_SKIPPED: break;
+    case REPEAT_REC_POOL: {
         const uint32_t need = std::max(sl.h_ctl->rec_alloc + sl.h_ctl->rec_alloc / 4 + 65536, sl.rec_cap);
         for (Slot &s : c->slot) {
             if (!s.allocated || s.rec_cap >= need) continue;
@@ -786,13 +788,17 @@ static int regrow(b200_demod_ctx *c, Slot &sl, int why) {
             if (dev_alloc(&s.d_rec_pool, s.rec_cap) != cudaSuccess || dev_alloc(&s.d_key_pool, s.rec_cap) != cudaSuccess)
                 return fail(c, B200_E_NOMEM, "cannot grow the record pool to %u records", need);
         }
-    } else if (why == 2) {       // a run of tiles with more live records than the per-warp staging areas hold: grow them to what it needs
+        break;
+    }
+    case REPEAT_STAGING: {       // a run of tiles with more live records than the per-warp staging areas hold: grow them to what it needs
         const uint32_t need = sl.h_ctl->stage_need + sl.h_ctl->stage_need / 8 + 64;
         cudaFree(c->d_stage_rec); cudaFree(c->d_stage_key); c->d_stage_rec = nullptr; c->d_stage_key = nullptr; c->stage_cap = 0;
         const size_t warps = (size_t)b200_scan_warps(c->n_sm);
         if (dev_alloc(&c->d_stage_rec, warps * need) != cudaSuccess || dev_alloc(&c->d_stage_key, warps * need) != cudaSuccess)
             return fail(c, B200_E_NOMEM, "cannot grow the record staging areas to %u records per warp", need);
         c->stage_cap = need;
+        break;
+    }
     }
     return B200_OK;
 }
@@ -805,7 +811,7 @@ static int execute_blocking(b200_demod_ctx *c, Slot &sl) {
         if (rc != B200_OK) return rc;
         rc = collect(c, sl, c->stream);
         if (rc <= 0) return rc;
-        rc = regrow(c, sl, rc);
+        rc = regrow(c, sl, (Repeat)rc);
         if (rc != B200_OK) return rc;
     }
     return fail(c, B200_E_NOMEM, "record pool still too small after regrowth");
@@ -1221,12 +1227,12 @@ API int b200_demod_wait(b200_demod_ctx *c) {
     if (!sl.completed) {                     // (completed: already repeated synchronously, see below)
         rc = collect(c, sl, c->res_stream);
         if (rc > 0) {
-            // This step (and therefore the ones behind it, which saw the failure flag of the step ahead and skipped their
+            // A Repeat: this step (and therefore the ones behind it, which saw the failure flag of the step ahead and skipped their
             // stage B) must be repeated.  Drain the pipeline and redo all of them, in order, synchronously.
-            for (int k = 1; k < c->n_flight; k++) CU(c, cudaEventSynchronize(c->slot[(idx + k) % NSLOT].ev[4]));
+            for (int k = 1; k < c->n_flight; k++) CU(c, cudaEventSynchronize(c->slot[(idx + k) % NSLOT].ev[3]));
             CU(c, cudaStreamSynchronize(c->stream));
             CU(c, cudaStreamSynchronize(c->res_stream));
-            rc = regrow(c, sl, rc);
+            rc = regrow(c, sl, (Repeat)rc);
             if (rc == B200_OK) rc = execute_blocking(c, sl);
             for (int k = 1; k < c->n_flight && rc == B200_OK; k++) {
                 Slot &next = c->slot[(idx + k) % NSLOT];

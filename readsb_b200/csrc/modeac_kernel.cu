@@ -11,6 +11,7 @@
 //   modeac_walk_kernel    the reference's sequential part, one warp per reference buffer (the skip state does not
 //                         survive a buffer): greedy walk over the bit map (a reply hides the next 69 positions), then
 //                         the lanes decode the accepted replies in parallel straight from the samples.
+//   ac_prefix_kernel, ac_pack_kernel, modeac_stats_kernel   after stage B: the reply lists packed in buffer order, receiver statistics.
 //
 // Exactness notes: float products and divisions are single IEEE operations (--fmad=false keeps them un-fused), the
 // sqrt(2) factors are fp64 exactly as the C expressions promote them, sqrt / sqrtf are the correctly rounded CUDA
@@ -160,7 +161,7 @@ __global__ void __launch_bounds__(AC2_WARPS * 32, 1) modeac_scan_kernel(const Ac
     extern __shared__ __align__(16) unsigned char ac_smem_raw[];
     Ac2Smem &S = *reinterpret_cast<Ac2Smem *>(ac_smem_raw);
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (P.ctl->overflow & 3u) return;
+    if (P.ctl->overflow & OV_STAGE_A_FAILED) return;
     {   // the folded table, once per CTA
         const uint4 *src = reinterpret_cast<const uint4 *>(P.tables->lut_fold);
         uint4 *dst = reinterpret_cast<uint4 *>(S.lut);
@@ -373,7 +374,7 @@ __global__ void __launch_bounds__(AC2_WARPS * 32, 1) modeac_scan_kernel(const Ac
 // ---- the sequential part, one warp per reference buffer ---------------------------------------------------------------
 __global__ void __launch_bounds__(256, 1) modeac_walk_kernel(const AcWalkParams P) {
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    if (P.ctl->overflow & 3u) return;
+    if (P.ctl->overflow & OV_STAGE_A_FAILED) return;
     for (uint32_t si = blockIdx.x; si < P.n_segs; si += gridDim.x) {
         const Segment seg = P.segs[si];
         const uint32_t stream_first_buf = P.segs[P.stream_seg_begin[seg.stream]].first_buf;
@@ -419,7 +420,7 @@ __global__ void __launch_bounds__(256, 1) modeac_walk_kernel(const AcWalkParams 
                     const uint32_t bal = __ballot_sync(FULLMASK, mine != 0xffffffffu);
                     if (!bal) break;
                     const uint32_t pos = __shfl_sync(FULLMASK, mine, __ffs(bal) - 1);
-                    if (lane == 0) { if (n < P.per_buf_cap) out[n].f1_sample = pos - xa; else atomicOr(&P.ctl->overflow, 32u); }
+                    if (lane == 0) { if (n < P.per_buf_cap) out[n].f1_sample = pos - xa; else atomicOr(&P.ctl->overflow, OV_MODEAC_CAP); }
                     n++;
                     next_ok = pos + AC_SKIP;
                 }
@@ -448,10 +449,36 @@ __global__ void __launch_bounds__(256, 1) modeac_walk_kernel(const AcWalkParams 
     }
 }
 
+// Exclusive prefix of the per-buffer reply counts (ac_pack_kernel packs the lists with it)
+__global__ void __launch_bounds__(1024) ac_prefix_kernel(const uint32_t *count, uint32_t *prefix, uint32_t n, const RunCtl *ctl) {
+    const uint32_t n_all = n;
+    __shared__ uint32_t scratch[40];
+    uint32_t base = 0;
+    if (ctl->overflow & RUN_REPEAT_BITS) n = 0;
+    for (uint32_t i0 = 0; i0 < n; i0 += blockDim.x) {
+        const uint32_t i = i0 + threadIdx.x;
+        const uint32_t v = i < n ? count[i] : 0;
+        uint32_t total;
+        const uint32_t ex = block_excl_scan(v, scratch, &total);
+        if (i < n) prefix[i] = base + ex;
+        base += total;
+    }
+    for (uint32_t i = n + threadIdx.x; i < n_all; i += blockDim.x) prefix[i] = base;
+    if (threadIdx.x == 0) prefix[n_all] = base;
+}
+
+// Pack the per-buffer reply lists in buffer order (one block per buffer).
+__global__ void ac_pack_kernel(const b200_modeac *ac_out, const uint32_t *count, const uint32_t *prefix, b200_modeac *packed, uint32_t cap, const RunCtl *ctl) {
+    if (ctl->overflow & RUN_REPEAT_BITS) return;          // the walk did not run (this step is going to be repeated): its counts are not this run's
+    const uint32_t s = blockIdx.x;
+    const uint32_t n = min(count[s], cap), base = prefix[s];
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) packed[base + i] = ac_out[(size_t)s * cap + i];
+}
+
 // after the count prefix: receiver statistics (the only state Mode A/C touches; skipped with the rest of stage B on a failed run)
 __global__ void modeac_stats_kernel(const AcWalkParams P, const uint32_t *prefix) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= P.n_streams || (P.ctl->overflow & (RUN_REPEAT_BITS | 32u))) return;
+    if (s >= P.n_streams || (P.ctl->overflow & (RUN_REPEAT_BITS | OV_MODEAC_CAP))) return;
     const uint32_t sb = P.stream_seg_begin[s], se = P.stream_seg_begin[s + 1];
     if (sb == se) return;
     const uint32_t b0 = P.segs[sb].first_buf, b1 = P.segs[se - 1].first_buf + P.segs[se - 1].n_bufs;
@@ -476,7 +503,11 @@ extern "C" int b200_launch_modeac(const AcScanParams *sp, const AcWalkParams *wp
     return (int)cudaGetLastError();
 }
 
-extern "C" int b200_launch_modeac_stats(const AcWalkParams *wp, const uint32_t *prefix, void *stream) {
+// After the Mode S stage B of the same step, on its stream: the walk's per-buffer reply lists -> one packed array in buffer order
+// (prefix, pack), then the receiver statistics.  Three launches.
+extern "C" int b200_launch_modeac_pack(const AcWalkParams *wp, uint32_t n_bufs, uint32_t *prefix, b200_modeac *packed, void *stream) {
+    ac_prefix_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(wp->ac_count, prefix, n_bufs, wp->ctl);
+    if (n_bufs) ac_pack_kernel<<<n_bufs, 32, 0, (cudaStream_t)stream>>>(wp->ac_out, wp->ac_count, prefix, packed, wp->per_buf_cap, wp->ctl);
     modeac_stats_kernel<<<(wp->n_streams + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*wp, prefix);
     return (int)cudaGetLastError();
 }

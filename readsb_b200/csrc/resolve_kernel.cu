@@ -1,6 +1,6 @@
-// resolve_kernel.cu — stage B and the frame finaliser.
+// resolve_kernel.cu — stage B, the frame finaliser and the ICAO filter's control kernels.
 //
-//   resolve_kernel  one warp per receiver: the sequential part of demodulate2400() (ICAO-filter dependent
+//   resolve_kernel  one CTA per receiver: the sequential part of demodulate2400() (ICAO-filter dependent
 //                   scoring mode_s.c:309-419, best-phase pick demod_2400.c:241-258, the accept test of
 //                   decodeModesMessage mode_s.c:443-596,:766-779, skip-ahead demod_2400.c:468, the filter flip
 //                   readsb.c:1227-1231), walked speculatively 32 candidates at a time with the receiver's two
@@ -308,7 +308,7 @@ __device__ __forceinline__ void resolve_buffer(const bool DEFER, const ResolvePa
                     *reinterpret_cast<uint16_t *>(&fr.pad_[0]) = (uint16_t)(si & 0xffffu);   // segment (low 16 bits) and data index
                     *reinterpret_cast<uint32_t *>(&fr.pad_[2]) = d;
                     fout[nframes] = fr;
-                } else atomicOr(&P.ctl->overflow, 4u);
+                } else atomicOr(&P.ctl->overflow, OV_FRAME_CAP);
                 if (corrected) c_acc1++; else c_acc0++;
                 c_bp[best_phase]++;
                 if (add) {
@@ -378,6 +378,26 @@ __device__ __noinline__ void resolve_buffer_call(bool defer, const ResolveParams
     resolve_buffer<BIG>(defer, P, S, R, out, seg, si, b, d_lo, d_hi, skip_in, seq, F, fout, fcap, lane);
 }
 
+// The capacity check of a receiver: stream_addable (scan kernel) bounds the insertions of this run; a generation never exceeds
+// (active now + that), so with 2 x that <= slots no table can fill up and stage B needs no overflow path.  A receiver that could
+// exceed it gets grow_log2 set and the run OV_FILTER_GROW: the host grows its tables and repeats.  True when the tables suffice.
+__device__ __forceinline__ bool tables_fit(const ResolveParams &P, StreamState *st, uint32_t log2, uint32_t g0, uint32_t g1, uint32_t add) {
+    const uint32_t need = max(g0, g1) + add;
+    if (2u * need <= (1u << log2)) return true;
+    uint32_t lg = log2 + 1;
+    while ((1u << lg) < 4u * need && lg < ICAO_MAXBITS + 1) lg++;
+    st->grow_log2 = lg;
+    atomicOr(&P.ctl->overflow, OV_FILTER_GROW);
+    return false;
+}
+
+// The asynchronous pipeline's "the step ahead has to be repeated" test: then this run is OV_SKIPPED.
+__device__ __forceinline__ bool step_ahead_repeats(const ResolveParams &P) {
+    if (!P.prev_stop || !*P.prev_stop) return false;
+    atomicOr(&P.ctl->overflow, OV_SKIPPED);
+    return true;
+}
+
 // COMPACT (the one-receiver kernel): the capacity check (capacity_check_all) is made here, by the CTA itself, while the other
 // threads already fetch the tables.  *n_frames_out (shared memory) receives the receiver's frame count, or ~0 when stage B must not run.
 template <bool BIG, bool COMPACT>
@@ -396,15 +416,8 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
             const uint32_t add = P.stream_addable[stream];
             P.stream_addable[stream] = 0;
             if (P.ctl->overflow & RUN_REPEAT_BITS) go = 0;
-            if (P.prev_stop && *P.prev_stop) { atomicOr(&P.ctl->overflow, 16u); go = 0; }
-            const uint32_t need = max(g0, g1) + add;
-            if (go && 2u * need > CAP) {
-                uint32_t lg = LOG2 + 1;
-                while ((1u << lg) < 4u * need && lg < ICAO_MAXBITS + 1) lg++;
-                st->grow_log2 = lg;
-                atomicOr(&P.ctl->overflow, 8u);
-                go = 0;
-            }
+            if (step_ahead_repeats(P)) go = 0;
+            if (go && !tables_fit(P, st, LOG2, g0, g1, add)) go = 0;
             *P.stop_out = go ? 0u : 1u;
             if (!go) *n_frames_out = ~0u;
         }
@@ -619,25 +632,17 @@ __device__ __forceinline__ void resolve_stream(const ResolveParams &P, ResolveSm
 // again, directly, with the filter as the reference would have it at that point.  In steady state (aircraft already
 // known, no flip) every speculation holds; the results are the sequential ones by construction either way.
 // When its receiver is resolved, the CTA reserves the receiver's range of the packed frame list and finalizes the frames into it.
-__device__ __forceinline__ void finalize_stream(const FinalizeParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane);
+__device__ __forceinline__ void finalize_stream(const ResolveParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane);
 
 // The capacity check of a run, for every receiver (the threads of one CTA share them): (1) the asynchronous pipeline's "the step
-// ahead has to be repeated" test; (2) the filter tables.  stream_addable[s] (scan kernel) bounds the insertions of this run; a
-// generation never exceeds (active now + that), so with 2 x that <= slots no table can fill up and stage B needs no overflow path.
-// A receiver that could exceed it gets grow_log2 set: the host grows its tables and repeats.
+// ahead has to be repeated" test; (2) the filter tables.
 __device__ __forceinline__ void capacity_check_all(const ResolveParams &P) {
-    if (threadIdx.x == 0 && P.prev_stop && *P.prev_stop) atomicOr(&P.ctl->overflow, 16u);
+    if (threadIdx.x == 0) step_ahead_repeats(P);
     for (uint32_t s = threadIdx.x; s < P.n_streams; s += blockDim.x) {
         const uint32_t add = P.stream_addable[s];
         P.stream_addable[s] = 0;
         StreamState *st = &P.state[s];
-        const uint32_t need = max(st->gen_count[0], st->gen_count[1]) + add;
-        if (2u * need > (1u << st->cap_log2)) {
-            uint32_t lg = st->cap_log2 + 1;
-            while ((1u << lg) < 4u * need && lg < ICAO_MAXBITS + 1) lg++;
-            st->grow_log2 = lg;
-            atomicOr(&P.ctl->overflow, 8u);
-        }
+        tables_fit(P, st, st->cap_log2, st->gen_count[0], st->gen_count[1], add);
     }
 }
 
@@ -684,7 +689,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32, RS_MIN_CTAS) resolve_kernel(con
     // asynchronous pipeline has to be repeated: leave every receiver's state untouched, report no frames; the host repairs and
     // repeats the run(s) in order.
     if (!stage_b_runs(P)) {
-        if (threadIdx.x == 0) { P.fin.frame_span[2 * stream] = 0; P.fin.frame_span[2 * stream + 1] = 0; }
+        if (threadIdx.x == 0) { P.frame_span[2 * stream] = 0; P.frame_span[2 * stream + 1] = 0; }
         return;
     }
     if ((st->cap_log2 != ICAO_CAP_LOG2) != BIG) return;
@@ -694,10 +699,10 @@ __global__ void __launch_bounds__(RS_WARPS * 32, RS_MIN_CTAS) resolve_kernel(con
     // depends on which CTA gets here first; frame_span tells every reader where each receiver's frames are.
     if (threadIdx.x == 0) {
         s_base = atomicAdd(&P.ctl->total_frames, s_nframes);
-        P.fin.frame_span[2 * stream] = s_base; P.fin.frame_span[2 * stream + 1] = s_nframes;
+        P.frame_span[2 * stream] = s_base; P.frame_span[2 * stream + 1] = s_nframes;
     }
     __syncthreads();
-    finalize_stream(P.fin, stream, s_base, s_nframes, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
+    finalize_stream(P, stream, s_base, s_nframes, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
 }
 
 __device__ __noinline__ void resolve_stream_big(const ResolveParams &P, ResolveSmem &S, StreamState *st, uint32_t stream, uint32_t *n_frames_out) { resolve_stream<true, true>(P, S, st, stream, n_frames_out); }
@@ -715,8 +720,8 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
     else resolve_stream_big(P, S, st, stream, &s_nframes);
     __syncthreads();
     const uint32_t n = s_nframes == ~0u ? 0u : s_nframes;         // ~0: stage B did not run (the step is going to be repeated)
-    if (threadIdx.x == 0) { P.fin.frame_span[0] = 0; P.fin.frame_span[1] = n; P.ctl->total_frames = n; }
-    finalize_stream(P.fin, stream, 0, n, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
+    if (threadIdx.x == 0) { P.frame_span[0] = 0; P.frame_span[1] = n; P.ctl->total_frames = n; }
+    finalize_stream(P, stream, 0, n, threadIdx.x >> 5, RS_WARPS, threadIdx.x & 31);
     if (P.carry_src && s_nframes != ~0u) {      // (not when the step is going to be repeated: it needs its halo again) every reader of this
                                                 // run's samples - scan kernel, finalizer above - is done: move the tail to the front
         __syncthreads();
@@ -732,31 +737,11 @@ __global__ void __launch_bounds__(RS_WARPS * 32, 1) resolve_solo_kernel(const __
     }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Mode A/C: exclusive prefix of the per-buffer reply counts (ac_pack_kernel packs the lists with it)
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) frame_prefix_kernel(const uint32_t *count, uint32_t *prefix, uint32_t n, const RunCtl *ctl) {
-    const uint32_t n_all = n;
-    __shared__ uint32_t scratch[40];
-    uint32_t base = 0;
-    if (ctl->overflow & RUN_REPEAT_BITS) n = 0;
-    for (uint32_t i0 = 0; i0 < n; i0 += blockDim.x) {
-        const uint32_t i = i0 + threadIdx.x;
-        const uint32_t v = i < n ? count[i] : 0;
-        uint32_t total;
-        const uint32_t ex = block_excl_scan(v, scratch, &total);
-        if (i < n) prefix[i] = base + ex;
-        base += total;
-    }
-    for (uint32_t i = n + threadIdx.x; i < n_all; i += blockDim.x) prefix[i] = base;
-    if (threadIdx.x == 0) prefix[n_all] = base;
-}
-
 __device__ __forceinline__ unsigned long long dmax_bits(double v) { return (unsigned long long)__double_as_longlong(v); }
 
 // One warp per accepted frame of receiver `stream`: the frame from its record, its signal power, the statistics (see the file
 // header).  Warp `warp` of `n_warps` takes frames warp, warp + n_warps, ... of the receiver's n and writes frame k to packed[base + k].
-__device__ __forceinline__ void finalize_stream(const FinalizeParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane) {
+__device__ __forceinline__ void finalize_stream(const ResolveParams &P, uint32_t stream, uint32_t base, uint32_t n, uint32_t warp, uint32_t n_warps, uint32_t lane) {
     for (uint32_t k = warp; k < n; k += n_warps) {
         const uint32_t fi = base + k;
         const b200_frame *src = &P.frames[(size_t)stream * P.frame_cap + k];
@@ -915,7 +900,7 @@ extern "C" int b200_prepare_resolve(void) {      // per device, from b200_demod_
     return (int)e;
 }
 
-// any_grown: some receiver of the context has filter tables of its own (then the second instantiation runs too; returns the launches made)
+// any_grown: some receiver of the context has filter tables of its own (then the second instantiation runs too)
 extern "C" int b200_launch_resolve(const ResolveParams *p, int any_grown, void *stream) {
     if (p->solo) {          // one receiver: capacity check, stage B, frame placement and finalizer in one launch
         resolve_solo_kernel<<<1, RS_WARPS * 32, sizeof(ResolveSmem), (cudaStream_t)stream>>>(*p);
@@ -933,21 +918,6 @@ extern "C" int b200_launch_init_state(StreamState *state, uint32_t n, uint32_t *
 
 extern "C" int b200_launch_icao_rehash(StreamState *state, uint32_t stream, uint32_t *new0, uint32_t *new1, uint32_t new_log2, void *cstream) {
     icao_rehash_kernel<<<1, 1024, 0, (cudaStream_t)cstream>>>(state, stream, new0, new1, new_log2);
-    return (int)cudaGetLastError();
-}
-
-// Mode A/C: pack the per-buffer reply lists in buffer order (prefix by frame_prefix_kernel, then one block per buffer).
-__global__ void ac_pack_kernel(const b200_modeac *ac_out, const uint32_t *count, const uint32_t *prefix, b200_modeac *packed, uint32_t cap, const RunCtl *ctl) {
-    if (ctl->overflow & RUN_REPEAT_BITS) return;          // the walk did not run (this step is going to be repeated): its counts are not this run's
-    const uint32_t s = blockIdx.x;
-    const uint32_t n = min(count[s], cap), base = prefix[s];
-    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) packed[base + i] = ac_out[(size_t)s * cap + i];
-}
-
-extern "C" int b200_launch_ac_pack(const b200_modeac *ac_out, const uint32_t *count, uint32_t *prefix, b200_modeac *packed, uint32_t n_units,
-                                   uint32_t cap, RunCtl *ctl, void *stream) {
-    frame_prefix_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(count, prefix, n_units, ctl);
-    if (n_units) ac_pack_kernel<<<n_units, 32, 0, (cudaStream_t)stream>>>(ac_out, count, prefix, packed, cap, ctl);
     return (int)cudaGetLastError();
 }
 

@@ -571,10 +571,10 @@ __device__ __noinline__ void finish_shared_tile(WarpSmem &W0, WarpSmem &W, const
     }
     if (wid == 0 && lane == 0) {
         uint32_t off = 0, ok = 1;
-        if (need > P.stage_cap) { atomicOr(&P.ctl->overflow, 2u); atomicMax(&P.ctl->stage_need, need); ok = 0; }         // as at the end of a whole-tile run
+        if (need > P.stage_cap) { atomicOr(&P.ctl->overflow, OV_STAGING_FULL); atomicMax(&P.ctl->stage_need, need); ok = 0; }         // as at the end of a whole-tile run
         else if (rec_tot) {
             off = atomicAdd(&P.ctl->rec_alloc, rec_tot);
-            if (off + rec_tot > P.rec_cap) { atomicOr(&P.ctl->overflow, 1u); ok = 0; }
+            if (off + rec_tot > P.rec_cap) { atomicOr(&P.ctl->overflow, OV_REC_POOL_FULL); ok = 0; }
         }
         S.sub_rec_off = off; S.sub_ok = ok;
     }
@@ -790,10 +790,10 @@ template <bool SUB, bool KEEP> __global__ void __maxnreg__(SC_MAXNREG) scan_kern
         if (SUB) { finish_shared_tile(F.w[0], W, P, lane, wid, n_stage); break; }
         uint32_t off = 0, ok = 1;
         if (lane == 0) {
-            if (n_stage > P.stage_cap) { atomicOr(&P.ctl->overflow, 2u); atomicMax(&P.ctl->stage_need, n_stage); ok = 0; }   // host grows the staging areas and reruns
+            if (n_stage > P.stage_cap) { atomicOr(&P.ctl->overflow, OV_STAGING_FULL); atomicMax(&P.ctl->stage_need, n_stage); ok = 0; }   // host grows the staging areas and reruns
             else if (n_stage) {
                 off = atomicAdd(&P.ctl->rec_alloc, n_stage);
-                if (off + n_stage > P.rec_cap) { atomicOr(&P.ctl->overflow, 1u); ok = 0; }                              // host regrows the pool and reruns
+                if (off + n_stage > P.rec_cap) { atomicOr(&P.ctl->overflow, OV_REC_POOL_FULL); ok = 0; }                              // host regrows the pool and reruns
             }
         }
         off = __shfl_sync(FULLMASK, off, 0); ok = __shfl_sync(FULLMASK, ok, 0);
