@@ -331,6 +331,28 @@ int b200_demod_get_stats(b200_demod_ctx *ctx, uint32_t stream, b200_demod_stats 
 #define B200_BEAST_MAX_RECORD 44
 int b200_demod_fetch_beast(b200_demod_ctx *ctx, uint32_t stream, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes);
 
+/* Raw (AVR) text records of the same frames and replies, encoded on the device, byte-identical to what readsb writes for them:
+ * by default the network record of modesSendRawOutput (net_io.c:1837-1863, a raw_out client / --net-ro-port), with
+ * B200_RAW_STDOUT the frame line of --raw on standard output (displayModesMessage, mode_s.c:1835-1841).
+ *   prefix   '*'; with B200_RAW_MLAT (Modes.mlat) and a non-zero timestamp '@' + "%012" PRIX64 of the 12 MHz timestamp.
+ *            A timestamp of 13 or more hex digits (>= 2^48, or negative, printed as unsigned) keeps only its first 12 digits
+ *            in the network record (the reference steps 13 bytes past the sprintf and the frame hex overwrites the rest);
+ *            the stdout line prints every digit.
+ *   frame    network: uppercase hex of the corrected frame, or with B200_RAW_VERBATIM (Modes.net_verbatim) of the bytes as
+ *            received; stdout: lowercase hex of the corrected frame.  A Mode A/C reply is two bytes (msgbits 16, mode_ac.c:171-173).
+ *   end      ";\n".
+ * Order, coverage and the cache of the encoded run are those of b200_demod_fetch_beast: the last run or the last completed
+ * step (also while the next asynchronous step is in flight), per buffer the Mode S frames then the Mode A/C replies; an absent
+ * receiver has 0 bytes.  The forwarding policy of outputMessage (first message of an aircraft held back, 2-bit repairs only
+ * with --net-verbatim, no MLAT-sourced frames) belongs to the tracker and is not applied: every accepted frame is encoded.
+ * *nbytes = size of the stream's records; B200_E_OVERFLOW if cap is smaller (nothing copied).  B200_E_INVAL for unknown flag
+ * bits and for B200_RAW_STDOUT | B200_RAW_VERBATIM (the stdout line always prints the corrected frame). */
+#define B200_RAW_MLAT       0x1u
+#define B200_RAW_VERBATIM   0x2u
+#define B200_RAW_STDOUT     0x4u
+#define B200_RAW_MAX_RECORD 48
+int b200_demod_fetch_raw(b200_demod_ctx *ctx, uint32_t stream, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes);
+
 /* ICAO address filter (icao_filter.h) — per stream, lives next to the resolver on the device.
  * Capacity: 2048 addresses per generation (two generations, entries live for one to two flip periods like the reference's).
  * The reference's tables grow instead (icao_filter.c:47-90, up to 2^20 buckets): a receiver never comes near the limit here

@@ -266,7 +266,9 @@ struct Sc16Params {
     float scale;                      // 1 / 32768 (sc16) or 1 / 2048 (sc16q11)
 };
 
-struct BeastParams {                 // beast_kernel.cu
+enum { ENC_BEAST = 0, ENC_RAW = 1 };
+
+struct EncodeParams {                // beast_kernel.cu: one wire format of a run's records
     const Segment *segs;
     const uint32_t *stream_seg_begin;
     const b200_frame *frames;         // packed (ResolveParams::packed)
@@ -278,7 +280,8 @@ struct BeastParams {                 // beast_kernel.cu
     uint32_t *stream_off, *stream_len;
     uint32_t *total;
     uint32_t cap;
-    uint32_t verbatim;
+    uint32_t format;                  // ENC_BEAST or ENC_RAW
+    uint32_t flags;                   // B200_BEAST_* or B200_RAW_* of the format
 };
 
 // ---- host-built constant tables, uploaded once ---------------------------------------------------
@@ -307,7 +310,7 @@ int b200_launch_icao_rehash(StreamState *state, uint32_t stream, uint32_t *new0,
 int b200_launch_modeac(const AcScanParams *sp, const AcWalkParams *wp, int n_sm, void *stream);
 int b200_prepare_convert(void);
 int b200_launch_sc16_convert(const Sc16Params *p, void *stream);
-int b200_launch_beast(const BeastParams *p, uint32_t n_streams, void *stream);
+int b200_launch_encode(const EncodeParams *p, uint32_t n_streams, void *stream);
 int b200_launch_modeac_pack(const AcWalkParams *wp, uint32_t n_bufs, uint32_t *prefix, b200_modeac *packed, void *stream);
 int b200_launch_icao_op(StreamState *state, uint32_t stream, int op, uint32_t addr, int *d_result, void *cstream);
 #ifdef __cplusplus

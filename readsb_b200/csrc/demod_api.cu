@@ -153,11 +153,11 @@ struct b200_demod_ctx {
     // scan kernel: per-warp staging of a run's live records, spill of the pre-check queue, ticks of the run in progress
     Rec *d_stage_rec = nullptr; uint32_t *d_stage_key = nullptr; uint16_t *d_q1_over = nullptr; uint32_t *d_tick_scratch = nullptr;
     uint32_t stage_cap = 0;
-    // Beast encoding (on demand, b200_demod_fetch_beast): packed records of every stream of one run
-    uint8_t *d_beast = nullptr, *h_beast = nullptr;
-    uint32_t *d_beast_meta = nullptr, *h_beast_meta = nullptr;   // [S] offsets, [S] lengths, [1] total
-    uint32_t beast_cap = 0;
-    int beast_slot = -1; uint32_t beast_flags = 0;               // which run the buffers hold
+    // Wire-format encoding (on demand, b200_demod_fetch_beast / _raw): packed records of every stream of one run in one format
+    uint8_t *d_enc = nullptr, *h_enc = nullptr;
+    uint32_t *d_enc_meta = nullptr, *h_enc_meta = nullptr;       // [S] offsets, [S] lengths, [1] total
+    uint32_t enc_cap = 0;
+    int enc_slot = -1; uint32_t enc_format = 0, enc_flags = 0;   // which run, format and flags the buffers hold
     // sc16 input: staging of one raw buffer, float sums of the buffers queued for the next run
     uint8_t *d_raw16 = nullptr;
     float2 *d_fsum = nullptr, *h_fsum = nullptr;
@@ -336,7 +336,7 @@ API void b200_demod_destroy(b200_demod_ctx *c) {
     cudaFreeHost(c->h_carry_src); cudaFreeHost(c->h_zero);
     cudaFree(c->d_raw16); cudaFree(c->d_fsum); cudaFreeHost(c->h_fsum);
     cudaFree(c->d_halo_store); cudaFree(c->d_halo_op); cudaFreeHost(c->h_halo_op);
-    cudaFree(c->d_beast); cudaFree(c->d_beast_meta); cudaFreeHost(c->h_beast); cudaFreeHost(c->h_beast_meta);
+    cudaFree(c->d_enc); cudaFree(c->d_enc_meta); cudaFreeHost(c->h_enc); cudaFreeHost(c->h_enc_meta);
     for (Slot &sl : c->slot) free_slot(sl);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     if (c->res_stream) cudaStreamDestroy(c->res_stream);
@@ -598,7 +598,7 @@ static int enqueue(b200_demod_ctx *c, Slot &sl, cudaStream_t scan, cudaStream_t 
     const bool one_seg = S == 1 && sl.nseg == 1 && !(c->cfg.flags & B200_CFG_MODE_AC) && scan == res;
     sl.desc_on_device = !one_seg;
     if (!one_seg) CU(c, cudaMemcpyAsync(sl.d_desc, sl.h_desc, sl.desc_bytes, cudaMemcpyHostToDevice, pre));
-    if (c->beast_slot == (int)(&sl - c->slot)) c->beast_slot = -1;      // the encoded records belong to the run being replaced
+    if (c->enc_slot == (int)(&sl - c->slot)) c->enc_slot = -1;          // the encoded records belong to the run being replaced
     // One receiver, no Mode A/C: the stage B kernel publishes the results into the host's (mapped) copy itself and zeroes the control
     // block and the per-buffer sums when it is done - no memset, no device-to-host copy in the stream.
     const bool publish = S == 1 && !(c->cfg.flags & B200_CFG_MODE_AC) && scan == res;
@@ -1279,53 +1279,68 @@ API int b200_demod_fetch_modeac(b200_demod_ctx *c, uint32_t s, b200_modeac *out,
     return B200_OK;
 }
 
-API int b200_demod_fetch_beast(b200_demod_ctx *c, uint32_t s, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes) {
-    if (!c || !nbytes || s >= c->cfg.n_streams || (flags & ~B200_BEAST_VERBATIM)) return B200_E_INVAL;
+// Encodes every stream of the current run in one wire format (once per run, format and flags: the buffers hold one) and copies
+// stream s's records out.
+static int fetch_encoded(b200_demod_ctx *c, uint32_t s, uint32_t format, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes) {
     // A later asynchronous step may be in flight: it works in the other slot, and this call only reads the completed one.
+    const char *what = format == ENC_RAW ? "raw" : "Beast";
     const uint32_t S = c->cfg.n_streams;
     Slot &sl = c->slot[c->cur];
-    if (c->beast_slot != c->cur || c->beast_flags != flags) {        // encode every stream of this run once
+    if (c->enc_slot != c->cur || c->enc_format != format || c->enc_flags != flags) {     // encode every stream of this run once
         CU(c, cudaSetDevice(c->device));
         const bool mode_ac = (c->cfg.flags & B200_CFG_MODE_AC) != 0;
         const uint64_t records = (uint64_t)sl.run_frames + (mode_ac ? sl.h_ac_prefix[sl.nbuf] : 0);
-        const uint64_t need = records * B200_BEAST_MAX_RECORD + 64;
-        if (need > 0xffffffffull) return fail(c, B200_E_OVERFLOW, "Beast output of one run exceeds 4 GiB");
-        if (!c->d_beast_meta) {
-            CU(c, dev_alloc(&c->d_beast_meta, 2 * S + 1));
-            CU(c, pin_alloc(&c->h_beast_meta, 2 * S + 1));
+        const uint64_t need = records * std::max(B200_BEAST_MAX_RECORD, B200_RAW_MAX_RECORD) + 64;    // one size serves both formats
+        if (need > 0xffffffffull) return fail(c, B200_E_OVERFLOW, "%s output of one run exceeds 4 GiB", what);
+        if (!c->d_enc_meta) {
+            CU(c, dev_alloc(&c->d_enc_meta, 2 * S + 1));
+            CU(c, pin_alloc(&c->h_enc_meta, 2 * S + 1));
         }
-        if (need > c->beast_cap) {
-            cudaFree(c->d_beast); cudaFreeHost(c->h_beast); c->d_beast = nullptr; c->h_beast = nullptr; c->beast_cap = 0;
+        if (need > c->enc_cap) {
+            cudaFree(c->d_enc); cudaFreeHost(c->h_enc); c->d_enc = nullptr; c->h_enc = nullptr; c->enc_cap = 0;
             const uint32_t cap2 = (uint32_t)std::min<uint64_t>(0xffffffffull, need + need / 2);
-            if (dev_alloc(&c->d_beast, cap2) != cudaSuccess || pin_alloc(&c->h_beast, cap2) != cudaSuccess)
-                return fail(c, B200_E_NOMEM, "cannot allocate %u bytes for the Beast output", cap2);
-            c->beast_cap = cap2;
+            if (dev_alloc(&c->d_enc, cap2) != cudaSuccess || pin_alloc(&c->h_enc, cap2) != cudaSuccess)
+                return fail(c, B200_E_NOMEM, "cannot allocate %u bytes for the %s output", cap2, what);
+            c->enc_cap = cap2;
         }
-        c->beast_slot = -1;
+        c->enc_slot = -1;
         cudaStream_t st = c->copy_stream;
         if (!sl.desc_on_device) { CU(c, cudaMemcpyAsync(sl.d_desc, sl.h_desc, sl.desc_bytes, cudaMemcpyHostToDevice, st)); sl.desc_on_device = true; }
-        CU(c, cudaMemsetAsync(c->d_beast_meta, 0, (2 * (size_t)S + 1) * 4, st));
-        BeastParams bp;
-        bp.segs = sl.d_segs; bp.stream_seg_begin = sl.d_stream_seg_begin; bp.frames = sl.d_packed; bp.frame_span = sl.d_frame_span;
-        bp.buf_out = sl.d_buf_out; bp.ac = mode_ac ? sl.d_ac_packed : nullptr; bp.ac_prefix = mode_ac ? sl.d_ac_prefix : nullptr;
-        bp.out = c->d_beast; bp.stream_off = c->d_beast_meta; bp.stream_len = c->d_beast_meta + S; bp.total = c->d_beast_meta + 2 * S;
-        bp.cap = c->beast_cap; bp.verbatim = (flags & B200_BEAST_VERBATIM) ? 1u : 0u;
-        { int r = b200_launch_beast(&bp, S, st); if (r) return fail(c, B200_E_CUDA, "beast launch: %s", cudaGetErrorString((cudaError_t)r)); }
-        CU(c, cudaMemcpyAsync(c->h_beast_meta, c->d_beast_meta, (2 * (size_t)S + 1) * 4, cudaMemcpyDeviceToHost, st));
+        CU(c, cudaMemsetAsync(c->d_enc_meta, 0, (2 * (size_t)S + 1) * 4, st));
+        EncodeParams ep;
+        ep.segs = sl.d_segs; ep.stream_seg_begin = sl.d_stream_seg_begin; ep.frames = sl.d_packed; ep.frame_span = sl.d_frame_span;
+        ep.buf_out = sl.d_buf_out; ep.ac = mode_ac ? sl.d_ac_packed : nullptr; ep.ac_prefix = mode_ac ? sl.d_ac_prefix : nullptr;
+        ep.out = c->d_enc; ep.stream_off = c->d_enc_meta; ep.stream_len = c->d_enc_meta + S; ep.total = c->d_enc_meta + 2 * S;
+        ep.cap = c->enc_cap; ep.format = format; ep.flags = flags;
+        { int r = b200_launch_encode(&ep, S, st); if (r) return fail(c, B200_E_CUDA, "%s encoder launch: %s", what, cudaGetErrorString((cudaError_t)r)); }
+        CU(c, cudaMemcpyAsync(c->h_enc_meta, c->d_enc_meta, (2 * (size_t)S + 1) * 4, cudaMemcpyDeviceToHost, st));
         CU(c, cudaStreamSynchronize(st));
-        const uint32_t total = c->h_beast_meta[2 * S];
-        if (total > c->beast_cap) return fail(c, B200_E_OVERFLOW, "Beast output larger than its worst case (%u > %u)", total, c->beast_cap);
+        const uint32_t total = c->h_enc_meta[2 * S];
+        if (total > c->enc_cap) return fail(c, B200_E_OVERFLOW, "%s output larger than its worst case (%u > %u)", what, total, c->enc_cap);
         if (total) {
-            CU(c, cudaMemcpyAsync(c->h_beast, c->d_beast, total, cudaMemcpyDeviceToHost, st));
+            CU(c, cudaMemcpyAsync(c->h_enc, c->d_enc, total, cudaMemcpyDeviceToHost, st));
             CU(c, cudaStreamSynchronize(st));
         }
-        c->beast_slot = c->cur; c->beast_flags = flags;
+        c->enc_slot = c->cur; c->enc_format = format; c->enc_flags = flags;
     }
-    const uint32_t off = c->h_beast_meta[s], len = c->h_beast_meta[S + s];
+    const uint32_t off = c->h_enc_meta[s], len = c->h_enc_meta[S + s];
     *nbytes = len;
-    if (len > cap) return fail(c, B200_E_OVERFLOW, "stream %u has %u bytes of Beast output, buffer holds %u", s, len, cap);
-    if (len) memcpy(out, c->h_beast + off, len);
+    if (len > cap) return fail(c, B200_E_OVERFLOW, "stream %u has %u bytes of %s output, buffer holds %u", s, len, what, cap);
+    if (len) memcpy(out, c->h_enc + off, len);
     return B200_OK;
+}
+
+API int b200_demod_fetch_beast(b200_demod_ctx *c, uint32_t s, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes) {
+    if (!c || !nbytes || s >= c->cfg.n_streams || (flags & ~B200_BEAST_VERBATIM)) return B200_E_INVAL;
+    return fetch_encoded(c, s, ENC_BEAST, flags, out, cap, nbytes);
+}
+
+API int b200_demod_fetch_raw(b200_demod_ctx *c, uint32_t s, uint32_t flags, uint8_t *out, uint32_t cap, uint32_t *nbytes) {
+    if (!c || !nbytes || s >= c->cfg.n_streams) return B200_E_INVAL;
+    if (flags & ~(B200_RAW_MLAT | B200_RAW_VERBATIM | B200_RAW_STDOUT)) return fail(c, B200_E_INVAL, "unknown raw flag bits 0x%x", flags);
+    if ((flags & B200_RAW_STDOUT) && (flags & B200_RAW_VERBATIM))
+        return fail(c, B200_E_INVAL, "B200_RAW_STDOUT prints the corrected frame: B200_RAW_VERBATIM does not apply");
+    return fetch_encoded(c, s, ENC_RAW, flags, out, cap, nbytes);
 }
 
 API int b200_demod_buffer_results(b200_demod_ctx *c, uint32_t s, b200_buffer_result *out, uint32_t cap, uint32_t *n) {

@@ -19,6 +19,9 @@ _LIB = None
 LIB_PATH = Path(__file__).resolve().parent / "libb200demod.so"
 
 
+RAW_MLAT, RAW_VERBATIM, RAW_STDOUT = 0x1, 0x2, 0x4     # b200_demod_fetch_raw flags (include/b200_demod.h)
+
+
 class DemodError(RuntimeError):
     pass
 
@@ -67,6 +70,7 @@ def lib():
         L.b200_demod_fetch_modeac.argtypes = [vp, u32, vp, u32, C.POINTER(u32)]
         L.b200_demod_submit_iq_sc16.argtypes = [vp, u32, vp, u32, C.c_int64, C.c_int]
         L.b200_demod_fetch_beast.argtypes = [vp, u32, u32, vp, u32, C.POINTER(u32)]
+        L.b200_demod_fetch_raw.argtypes = [vp, u32, u32, vp, u32, C.POINTER(u32)]
         L.b200_demod_buffer_results.argtypes = [vp, u32, vp, u32, C.POINTER(u32)]
         L.b200_demod_total_frames.argtypes = [vp, C.POINTER(u64)]
         L.b200_demod_get_stats.argtypes = [vp, u32, C.POINTER(Stats)]
@@ -92,6 +96,7 @@ EXPORTED_SYMBOLS = [
     "b200_demod_submit_mag_u16_levels", "b200_demod_set_preamble_threshold",
     "b200_demod_run_device_sc16", "b200_demod_run_device_sc16_async", "b200_demod_run_host_sc16_async",
     "b200_demod_run_device_rx", "b200_demod_run_device_rx_async", "b200_demod_run_host_rx_async", "b200_demod_restart_stream",
+    "b200_demod_fetch_raw",
 ]
 
 
@@ -281,6 +286,20 @@ class Demodulator:
             return b""
         buf = (C.c_uint8 * n.value)()
         self._check(self.L.b200_demod_fetch_beast(self.h, stream, flags, buf, n.value, C.byref(n)))
+        return bytes(buf)
+
+    def raw(self, stream: int, mlat: bool = False, verbatim: bool = False, stdout: bool = False) -> bytes:
+        """Raw / AVR text records of the last run's frames (+ Mode A/C replies) of one stream: the network record of
+        modesSendRawOutput (net_io.c:1837-1863), or with stdout=True the --raw line of displayModesMessage (mode_s.c:1835-1841).
+        mlat: '@' + 12 MHz timestamp instead of '*' (--mlat); verbatim: bytes as received (--net-verbatim, network form only)."""
+        n = C.c_uint32()
+        flags = (RAW_MLAT if mlat else 0) | (RAW_VERBATIM if verbatim else 0) | (RAW_STDOUT if stdout else 0)
+        rc = self.L.b200_demod_fetch_raw(self.h, stream, flags, None, 0, C.byref(n))
+        if n.value == 0:
+            self._check(rc)
+            return b""
+        buf = (C.c_uint8 * n.value)()
+        self._check(self.L.b200_demod_fetch_raw(self.h, stream, flags, buf, n.value, C.byref(n)))
         return bytes(buf)
 
     def stats(self, stream: int) -> dict:
